@@ -41,17 +41,17 @@ METRIC = "blob hash-and-cache throughput"
 UNIT = "GB/s"
 
 WORKLOADS = {
-    # BASELINE.json configs[2]: 256 concurrent 64 MB HF LFS range streams on 1 B200
+    # BASELINE.json configs[2]: 256 concurrent 64 MB HF LFS range streams on 1 GPU
     "hf_lfs_256x64MiB": {"sizes": [64 << 20] * 256, "baseline_config": 2},
     # BASELINE.json configs[1]: Llama-3-8B safetensors shard set (real shard sizes, SURVEY.md §8d)
     "llama3_8b_shards": {"sizes": [4976698672, 4999802720, 4915916176, 1168138808], "baseline_config": 1},
     # kernel saturation probe (not a BASELINE config): enough streams to fill every sub-partition
-    # 148 SMs x 4 sub-partitions x 8 warps x 32 lanes = 151552 streams
-    "saturate_151552x112KiB": {"sizes": [112 << 10] * 151552, "baseline_config": None},
+    # 132 SMs x 4 sub-partitions x 8 warps x 32 lanes = 135168 streams (15.1 GB: one copy in HBM plus its CAS copy fit 80 GB)
+    "saturate_135168x112KiB": {"sizes": [112 << 10] * 135168, "baseline_config": None},
     "tiny": {"sizes": [1 << 20] * 64, "baseline_config": None},
     # BASELINE.json configs[3]: Ollama manifest + 7B GGUF layer blobs (SURVEY.md section 8d sizes: model layer of a
     # typical 7B Q4_0, license, params, config), digest verify sharded by dm_shard_of over the ranks
-    # (4 B200 in the config).  One layer dominates: one chain on one GPU, whatever N is.
+    # (4 GPUs in the config).  One layer dominates: one chain on one GPU, whatever N is.
     "ollama_7b_manifest": {"sizes": [3826793677, 11357, 17, 420], "baseline_config": 3, "routing": "digest"},
     # BASELINE.json configs[4]: blob-size sweep, scaled DOWN and saying so: classes 1 MiB .. 1 GiB in x4 steps
     # (the config's 64 GiB top class is one 14-minute serial chain on any number of GPUs), 2 GiB per class per
@@ -68,7 +68,7 @@ def _peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s; not measured)"
 
 
 def _cpu_quota():
@@ -92,23 +92,23 @@ def _cfs_throttle():
 
 def _kernel_for(n):
     """Mirror of streams_per_warp_for() in demodel_b200/csrc/sha256_kernels.cuh (for the report only)."""
-    for limit, name in ((296, "deep (1 stream/warp pair)"), (592, "group (2 streams/warp pair)"), (1184, "group (4 streams/warp pair)"),
-                        (2368, "group (8 streams/warp pair)"), (4736, "group (16 streams/warp pair)"), (9472, "group (16 streams/warp)")):
+    for limit, name in ((264, "deep (1 stream/warp pair)"), (528, "group (2 streams/warp pair)"), (1056, "group (4 streams/warp pair)"),
+                        (2112, "group (8 streams/warp pair)"), (4224, "group (16 streams/warp pair)"), (8448, "group (16 streams/warp)")):
         if n <= limit:
             return name
     return "wide (32 streams/warp)"
 
 
 def _int_issue_roofline(n_streams, hashed_gbs, sm_mhz):
-    """The bound that actually binds SHA-256 on sm_100a (DESIGN.md section 5, profiles/r01_ubench_issue_rates.txt):
-    the ALU pipe takes one warp-instruction per 2 cycles per sub-partition.  Chip ceiling: >= 1040 ALU-pipe
-    instructions per 64-byte block per warp of 32 lanes on 592 sub-partitions.  Few streams: one warp per
+    """The bound that actually binds SHA-256 on sm_90a (DESIGN.md section 5): the ALU pipe takes one
+    warp-instruction per 2 cycles per sub-partition.  Chip ceiling: >= 1040 ALU-pipe
+    instructions per 64-byte block per warp of 32 lanes on 528 sub-partitions (132 SMs).  Few streams: one warp per
     stream needs the round's six rotations and four boolean functions on that pipe whatever is done with the
     additions = 20 cycles per round, 64 rounds per 64 bytes (the shipped round form issues 11: 22 cycles).
     Reported beside the HBM roofline the metric asks for; never raises."""
     try:
-        ghz = (sm_mhz or 1965.0) / 1e3
-        chip = 592 * ghz * (32 * 64) / (1040 * 2)                 # GB/s
+        ghz = (sm_mhz or 1980.0) / 1e3                            # H100 SXM maximum SM clock when not sampled
+        chip = 528 * ghz * (32 * 64) / (1040 * 2)                 # GB/s
         per_stream = ghz / 20.0                                    # GB/s: 1 byte per round
         peak = min(chip, n_streams * per_stream)
         return {"bound": "int32 ALU-pipe issue", "peak": peak, "achieved": hashed_gbs, "frac": hashed_gbs / peak, "unit": "GB/s hashed",
@@ -141,6 +141,43 @@ def _numa_bind(local_rank):
         return {"gpu_bus": bus, "numa_node": node, "cpus": len(cpus)}
     except Exception:
         return None
+
+
+DUMP_BUDGET = 64 << 20          # bytes of .npy payload in all
+
+
+def _dump_outputs(out_dir, eng, digests, matched, sizes, hash_only):
+    """What the last timed dm_ingest_device step handed back - the digest bytes (blob x 32) and the per-blob verdicts
+    - plus, unless --hash-only, a sample of the CAS copies the same step wrote, read back through dm_cache_read: one
+    4 KiB window per sampled blob at a seeded offset.  Everything as float32 (each value is a byte or 0/1).  Blobs
+    beyond the budget are sampled with a fixed seed; `blob_index` names the rows."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(sizes)
+    digs = np.asarray(digests, dtype=np.uint8).reshape(n, 32)
+    rng = np.random.default_rng(SEED)
+    rows = min(n, (DUMP_BUDGET // 2) // (4 * 34))
+    idx = np.arange(n) if rows == n else np.sort(rng.choice(n, size=rows, replace=False))
+    np.save(os.path.join(out_dir, "blob_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "digests.npy"), digs[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "matched.npy"), np.asarray(matched, dtype=np.float32).reshape(n)[idx])
+    if hash_only:
+        return
+    win = 4096
+    k = min(n, (DUMP_BUDGET // 2) // (4 * win))
+    pick = np.sort(rng.choice(n, size=k, replace=False)) if k < n else np.arange(n)
+    cas = np.zeros((k, win), dtype=np.float32)
+    lo = np.zeros(k, dtype=np.float64)
+    for r, i in enumerate(pick):
+        size = int(sizes[i])
+        lo[r] = int(rng.integers(0, max(size - win, 0) + 1))
+        rid, _ = eng.cache_open(digs[i].tobytes())
+        got = np.frombuffer(eng.cache_read(rid, int(lo[r]), min(win, size)), dtype=np.uint8)
+        eng.cache_close(rid)
+        cas[r, :got.size] = got
+    np.save(os.path.join(out_dir, "cas_sample_blob.npy"), pick.astype(np.float64))
+    np.save(os.path.join(out_dir, "cas_sample_offset.npy"), lo)
+    np.save(os.path.join(out_dir, "cas_sample.npy"), cas)
 
 
 def _layout(sizes):
@@ -201,7 +238,7 @@ def _digest_routed_set(eng, torch, dist, n_total, size_of, rank, world, local, b
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi sampling DURING the timed region (clocks, power, throttle reasons)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -333,6 +370,9 @@ def main():
     ap.add_argument("--cas-slack-mib", type=int, default=4096, help="HBM arena beyond one copy of the workload (ring-path bodies, probes)")
     ap.add_argument("--blobs", type=int, default=0, help="override: number of blobs (with --blob-bytes)")
     ap.add_argument("--blob-bytes", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (digests, verdicts) and a seeded sample of the CAS "
+                         "copies it wrote as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
     if args.blobs and args.blob_bytes:
         args.workload = f"custom_{args.blobs}x{args.blob_bytes}"
@@ -427,6 +467,8 @@ def main():
     s1 = eng.stats()
     assert np.array_equal(d, expect_arr) and m.all()
     launches = int(s1["kernel_launches"] - s0["kernel_launches"])
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, eng, d, m, sizes, args.hash_only)
 
     tt = torch.tensor([wall, kernel_ms], dtype=torch.float64, device=f"cuda:{local}")
     if world > 1:
@@ -476,7 +518,8 @@ def main():
     probes = None
     if rank == 0 and not args.no_probes and args.blobs == 0 and routing == "url" and not wl.get("classes"):
         probes = {}
-        for name, pn, pbytes in (("wide_151552_streams", 151552, 16384), ("group8_4096_streams", 4096, 524288)):
+        alu_bound = _int_issue_roofline(1 << 30, 0.0, (clocks or {}).get("sm_mhz"))["chip_ceiling"]     # GB/s hashed
+        for name, pn, pbytes in (("wide_135168_streams", 135168, 16384), ("group16_4096_streams", 4096, 524288)):
             po = np.arange(pn, dtype=np.uint64) * np.uint64(pbytes)
             pl = np.full(pn, pbytes, dtype=np.uint64)
             pdev = torch.empty(pn * pbytes, dtype=torch.uint8, device=f"cuda:{local}")
@@ -494,7 +537,7 @@ def main():
             probes[name] = {"streams": pn, "blob_bytes": pbytes, "kernel_ms": k_ms, "hashed_GBps": ach / 2,
                             "roofline": {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
                                          "frac": ach / hbm_peak, "algorithmic_bytes_per_blob_byte": 2},
-                            "alu_issue_bound_GBps": 1146.0, "frac_of_alu_bound": ach / 2 / 1146.0}
+                            "alu_issue_bound_GBps": alu_bound, "frac_of_alu_bound": ach / 2 / alu_bound}
             import ctypes as _C
             lib_ = demodel_b200.load()
             for i_ in range(pn):                                # drop the probe's blobs from the CAS
@@ -503,7 +546,7 @@ def main():
 
     # small-blob latency through the stream API: open -> write 4 KiB -> finish (DMA + launch + digest back)
     if probes is not None:
-        small = np.frombuffer(os.urandom(4096), dtype=np.uint8)
+        small = np.random.default_rng(SEED).integers(0, 256, size=4096, dtype=np.uint8)
         lat = []
         for it in range(220):
             t0_ = time.perf_counter()
@@ -531,7 +574,7 @@ def main():
         # CUDA driver's threads and the DMA submissions share the same cgroup quota)
         # ... and the ranks of one node share it, so each takes its 1/world share.
         drive_threads = max(1, min(conc, args.e2e_threads or max(1, ncpu_eff // (2 * world))))
-        e2e_steps = max(1, min(args.steps, 3))
+        e2e_steps = max(1, args.steps)
         for _ in range(1):
             dd, mm, _ = eng.proxy_drive(host, hoff, expect=expect, chunk=32768, concurrency=conc,
                                         nthreads=drive_threads, zero_copy=args.e2e_zero_copy)
@@ -613,7 +656,7 @@ def main():
         agree = torch.tensor([ready], dtype=torch.float64, device=f"cuda:{local}")
         dist.all_reduce(agree, op=dist.ReduceOp.MIN)
         if float(agree[0]) > 0:
-            f_steps = max(1, min(args.steps, 3))
+            f_steps = max(1, args.steps)
             barrier()
             t0 = time.perf_counter()
             fk = 0.0
@@ -632,7 +675,7 @@ def main():
                         "value": fbytes * f_steps / float(tf[0]) / 1e9, "unit": UNIT, "ms_per_step": 1e3 * float(tf[0]) / f_steps,
                         "kernel_ms_per_step_max_rank": float(tf[1]) / f_steps,
                         "note": "warp-per-stream regime: a rank's time is its longest chain, not its blob count, while it holds "
-                                "<= 592 streams (one per sub-partition) - the imbalance costs HBM, not time"}
+                                "<= 528 streams (one per sub-partition) - the imbalance costs HBM, not time"}
         elif sharding is None:
             sharding = {"error": "another rank could not set up its share", "blobs_per_rank": counts}
         for i in owned:
@@ -684,22 +727,11 @@ def main():
         del src, cache
 
     if rank == 0:
-        # roofline.traffic: dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel, from an
-        # ncu capture of this workload (tools/prof_default.sh writes profiles/roofline_traffic.json).  It is only
-        # reported when the capture was taken with the kernel variant that ran here.
+        # roofline.traffic (DRAM bytes of one launch, from a hardware-counter capture) is not measured: no capture of
+        # this build is stored.
         traffic, traffic_src = None, None
         lib_ = demodel_b200.load()
         variant_now = os.environ.get("DM_KERNEL_VARIANT") or f"{lib_.dm_default_kernel_variant(0)},{lib_.dm_default_kernel_variant(1)}"
-        tpath = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-        if os.path.exists(tpath) and not (args.hash_only or args.kernel):
-            try:
-                ent = json.load(open(tpath)).get(args.workload)
-                # the capture is of ONE kernel family: only that half of "wide,deep" has to match what ran
-                half = 0 if isinstance(ent, dict) and ent.get("family") == "wide" else 1
-                if isinstance(ent, dict) and ent.get("kernel_variant", "").split(",")[half:half + 1] == variant_now.split(",")[half:half + 1]:
-                    traffic, traffic_src = ent["bytes"], ent.get("source")
-            except Exception:
-                traffic = None
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": 1e3 * wall_max / args.steps, "higher_is_better": True, "scaling": "strong" if routing == "digest" else "weak",
@@ -708,7 +740,7 @@ def main():
             "config": {"workload": args.workload, "baseline_config": WORKLOADS[args.workload]["baseline_config"],
                        "blobs_per_gpu": n, "bytes_per_gpu_per_step": total, "mode": "hash-only" if args.hash_only else "hash-and-cache (fused CAS copy)",
                        "kernel": args.kernel or _kernel_for(n), "seed": hex(SEED),
-                       "l2": "inputs (%.1f GB) larger than L2 (126 MB); no flush needed" % (total / 1e9),
+                       "l2": "inputs (%.1f GB) %s than L2 (50 MB)" % (total / 1e9, "larger" if total > 50e6 else "NOT larger"),
                        "parallelism": (f"shard{world} (fixed set routed by dm_shard_of(digest), no collective)" if routing == "digest"
                                        else f"shard{world} (URL-hash homed, no collective)"),
                        "blobs_per_rank": shard_counts, "scaled": wl.get("scaled"), "job_bytes_per_step": job_total},
@@ -722,8 +754,8 @@ def main():
                 "workload_choice": "BASELINE configs[2] (256 x 64 MiB, 17.18 GB) is the largest single-GPU configuration; "
                                    "configs[1] (4 Llama-3-8B shards, 16.06 GB) is selectable with --workload llama3_8b_shards",
                 "configs1_expectation": "SHA-256 chains block to block, so 4 blobs are 4 serial chains: --workload llama3_8b_shards "
-                                        "measured 0.2455 GB/s (65.4 s per pass: the 5.0 GB shard at 76.4 MB/s), CPU arm 5.35 GB/s on 4 cores",
-                "binding_bound": "integer ALU issue (~1.15 TB/s per B200 for SHA-256), not HBM; see DESIGN.md section 5",
+                                        "takes as long as its 5.0 GB shard at one stream's rate",
+                "binding_bound": "integer ALU issue (roofline.int_issue.chip_ceiling for SHA-256), not HBM; see DESIGN.md section 5",
             },
             "host": {"cpus": os.cpu_count(), "cpu_quota": _cpu_quota(), "kernel_variant": os.environ.get("DM_KERNEL_VARIANT"),
                      "numa_bind": numa},

@@ -1,6 +1,6 @@
-"""demodel_b200 — B200-native blob hash-and-cache engine (host-side mirror).
+"""demodel_b200 — H100-native blob hash-and-cache engine (host-side mirror).
 
-The product is ``libdemodel_b200.so`` (hand-written sm_100a SHA-256 kernels +
+The product is ``libdemodel_b200.so`` (hand-written sm_90a SHA-256 kernels +
 the ingest/CAS engine behind the C-ABI in ``include/demodel_b200.h``).  The
 Python here is a thin ctypes mirror for tests and the benchmark; it never
 computes a digest itself and it fails loudly when the library is missing.

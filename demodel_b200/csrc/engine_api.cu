@@ -244,7 +244,8 @@ static int engine_create(const dm_config *cfg, dm_engine **out)
     cudaDeviceProp prop;
     CU_INIT(cudaGetDeviceProperties(&prop, e->device));
     e->sm_count = prop.multiProcessorCount;
-    if (prop.major < 10) { fail(DM_ENODEV, "kernels are built for sm_100a only"); dm_engine_destroy(e); return DM_ENODEV; }
+    // sm_90a SASS (no PTX in the fat binary) loads on compute capability 9.0 only
+    if (prop.major != 9 || prop.minor != 0) { fail(DM_ENODEV, "kernels are built for sm_90a only"); dm_engine_destroy(e); return DM_ENODEV; }
 
     for (int i = 0; i < kCopyStreams; ++i) CU_INIT(cudaStreamCreateWithFlags(&e->copy_stream[i], cudaStreamNonBlocking));
     CU_INIT(cudaStreamCreateWithFlags(&e->ingest_stream, cudaStreamNonBlocking));

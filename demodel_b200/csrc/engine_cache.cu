@@ -639,7 +639,7 @@ static int ingest_device_impl(dm_engine *e, const void *dev_base, const uint64_t
     }
     const uint32_t n_rest = n - n_long;
     // the two launches of a split batch share the chip: the rest runs one warp per group (the long jobs keep their
-    // warp pairs while there are at most 296 of them)
+    // warp pairs while there are at most kMaxWarpPairs of them)
     const int spw_rest = n_long ? dm::streams_per_warp_unpaired(n_rest) : spw;
     const int v_rest = n_long && e->variant_deep >= 8 ? 7 : e->variant_deep;
     // Very large lane-per-stream batches go out in chunks, each on a stream of its own: at 10^5 blobs the host work

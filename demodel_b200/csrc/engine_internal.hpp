@@ -252,7 +252,7 @@ struct dm_engine {
     dm_config cfg{};
     std::string cas_dir;
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int numa_node = -1;              // DM_F_NUMA_LOCAL: the node the engine bound itself to, -1 = not bound
     int force_spw = 0;               // DM_FORCE_SPW: 1/2/4/8/16/32 streams per warp for every launch (tuning only)
     int variant_wide = dm::kDefaultWideVariant, variant_deep = dm::kDefaultDeepVariant;   // DM_KERNEL_VARIANT overrides (tuning only)

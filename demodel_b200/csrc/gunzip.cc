@@ -1,7 +1,7 @@
 // dm_gunzip: inflate a gzip (RFC 1952) or zlib (RFC 1950) body - host code, no dependencies.
 //
 // Why it is on this path: registries answer manifest requests with `Content-Encoding: gzip`, and the one
-// cached body the reference documents is exactly that (/root/reference/CONTRIBUTING.md:76-99 is the hexdump,
+// cached body the reference documents is exactly that (demodel/CONTRIBUTING.md:76-99 is the hexdump,
 // :116 says the cache kept it encoded).  The manifest hook (dm_manifest_parse -> dm_manifest_prefetch) needs
 // the JSON, so the tee inflates such a body first.  Blob bodies themselves (LFS files, OCI layers) are
 // served identity-encoded and never come through here.

@@ -2,7 +2,7 @@
 // every layer blob with its sha256 digest and size *before* the bodies are
 // requested, so the proxy can pre-open one verified stream per layer.
 //
-// Manifest shape: /root/reference/CONTRIBUTING.md:128-153 (the decoded body of
+// Manifest shape: demodel/CONTRIBUTING.md:128-153 (the decoded body of
 // the reference's one cached fixture) — {"config": {descriptor}, "layers":
 // [{descriptor}, ...]} with descriptor = {"mediaType", "digest": "sha256:<hex>",
 // "size"}.  The parser below is a small JSON walker that collects every object

@@ -2,7 +2,7 @@
 // restated as C++ threads over the hook wrappers in proxy_hooks.hpp.
 //
 // In the reference, net/http runs one goroutine per client connection
-// (/root/reference/cmd/demodel/start.go:210-215) and goproxy reads the
+// (demodel/cmd/demodel/start.go:210-215) and goproxy reads the
 // response body on that goroutine in 32 KiB pieces.  Here `nthreads` OS
 // threads play `concurrency` such goroutines the way the Go scheduler runs
 // them on GOMAXPROCS threads: each thread round-robins one piece at a time

@@ -5,7 +5,7 @@
 // the parity tests drive these instead.
 //
 //   BodyTee    — installed by the OnResponse hook around resp.Body
-//                (/root/reference/cmd/demodel/start.go:201-204 returns resp
+//                (demodel/cmd/demodel/start.go:201-204 returns resp
 //                unchanged today).  Read(p) reads from upstream, tees the
 //                bytes into the engine, returns them to goproxy's copy loop;
 //                at EOF it finishes the stream and records the verdict;

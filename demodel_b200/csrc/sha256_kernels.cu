@@ -1,8 +1,8 @@
-// Multi-buffer SHA-256 for sm_100a: the hot path of the blob hash-and-cache
+// Multi-buffer SHA-256 for sm_90a (H100): the hot path of the blob hash-and-cache
 // engine.  Pure 32-bit integer work (SHF / LOP3 / IADD3 / IMAD) — no tensor
 // cores, no floating point.  Three kernel shapes share the round function;
 // the engine picks one per launch from the number of co-resident streams
-// (streams_per_warp_for, crossovers measured on B200):
+// (streams_per_warp_for):
 //
 //   sha256_wide_kernel   one 32-bit lane per live stream (the multi-buffer
 //                        form north_star describes): W[16] and the eight
@@ -11,10 +11,11 @@
 //                        shipped variant rolls the rounds 16 at a time (round
 //                        constants from the constant bank; the fully unrolled
 //                        form stalled on the instruction cache), issues the
-//                        additions on the FMA pipe, and stages every lane's next
-//                        line in shared memory with cp.async.  Bound by the ALU
+//                        additions on the FMA pipe and loads each line into
+//                        registers (style 2; style 5 stages it in shared memory
+//                        with cp.async, slower on H100).  Bound by the ALU
 //                        pipe (one warp-instruction per 2 cycles per
-//                        sub-partition): <= 1.15 TB/s per B200, 1.02 measured;
+//                        sub-partition): <= ~1.0 TB/s on 132 SMs at 1.98 GHz;
 //                        needs > ~10^4 streams to fill the chip.
 //   sha256_deep_kernel   one warp per stream, for few live streams.  SHA-256's
 //                        serial chain is only the 64 rounds; the message
@@ -23,11 +24,11 @@
 //                        (coalesced 2 KiB load) and stage W[t]+K[t] in shared
 //                        memory; then the warp runs the 32x64 dependent rounds
 //                        reading one broadcast LDS.128 per 4 rounds.  ~1.9x the
-//                        per-stream rate of the lane-per-stream form (76 MB/s).
+//                        per-stream rate of the lane-per-stream form.
 //   sha256_group_kernel  S = 2/4/8/16 streams per warp: the deep kernel's two
 //                        phases with lane = block_slot * S + stream, so S round
-//                        chains advance per instruction.  Wins between 593 and
-//                        ~9 500 streams (S = the smallest that keeps one warp per
+//                        chains advance per instruction.  Wins between 265 and
+//                        ~8 500 streams (S = the smallest that keeps one warp per
 //                        sub-partition).
 //
 // All optionally write every byte they read to `dst` (the blob's CAS
@@ -36,7 +37,7 @@
 //
 // The digest definition is FIPS 180-4 (what Go crypto/sha256 implements —
 // the reference names it in BASELINE.json north_star but holds no call site:
-// /root/reference/cmd/demodel/start.go:201-204 returns resp unchanged).
+// the reference's cmd/demodel/start.go:201-204 returns resp unchanged).
 #include "sha256_kernels.cuh"
 #include "blobgen.h"
 #include "sha256_round.cuh"
@@ -388,7 +389,7 @@ __device__ __forceinline__ void expand_schedule(uint32_t (&w)[16], uint4 *out)
 // deep: one warp per stream
 // ---------------------------------------------------------------------------
 constexpr int kDeepWarps = 1;                 // warps per CTA; 1 lets the block scheduler
-                                              // spread few streams over all 592 sub-partitions
+                                              // spread few streams over all 528 sub-partitions
 constexpr int kKwStride = 68;                 // words per staged block: 64 + 4 pad -> conflict-free STS.128
 
 template <int kFma>
@@ -469,7 +470,7 @@ sha256_deep_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *_
 // ---------------------------------------------------------------------------
 // deep2: two warps per stream - a schedule warp runs ahead of the round warp
 // ---------------------------------------------------------------------------
-// With at most 296 live streams (half the sub-partitions) every stream can have TWO warps, each on a sub-partition
+// With at most 264 live streams (half the sub-partitions) every stream can have TWO warps, each on a sub-partition
 // of its own.  The serial chain stays what it is - 64 dependent rounds per block on one warp - but everything else
 // leaves that warp: warp 1 loads the next 32 blocks, stores the fused CAS copy and expands the 32 message
 // schedules into the other half of a double-buffered W+K stage while warp 0 is still running the rounds of the
@@ -861,7 +862,7 @@ cudaError_t launch_sha256_deep(const HashJob *jobs, uint32_t njobs, uint32_t *st
     clear_stale_error();
     if (variant == 9) variant = 8;                     // (9 = two-warp group kernels too; the deep kernel's own rule is 8's)
     if (variant == 8 && njobs > kMaxWarpPairs) variant = 7;
-    if (variant == 10) variant = 8;                    // 10 = two warps per stream whatever the count (A/B of the 296 rule)      // two warps per stream only while each still gets a sub-partition of its own
+    if (variant == 10) variant = 8;                    // 10 = two warps per stream whatever the count (A/B of the 264 rule)      // two warps per stream only while each still gets a sub-partition of its own
     switch (variant) {
     case 1: case 3: sha256_deep_kernel<1><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
     case 2: sha256_deep_kernel<2><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
@@ -870,7 +871,7 @@ cudaError_t launch_sha256_deep(const HashJob *jobs, uint32_t njobs, uint32_t *st
     case 6: sha256_deep_kernel<6><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
     case 7: sha256_deep_kernel<7><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
     // 8: form 7 with a schedule warp running ahead of the round warp (two warps per stream; callers keep it to
-    //    launches of at most 296 jobs, so that every warp has a sub-partition of its own)
+    //    launches of at most 264 jobs, so that every warp has a sub-partition of its own)
     case 8: sha256_deep2_kernel<7><<<njobs, 64, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
     default: sha256_deep_kernel<0><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
     }
@@ -935,7 +936,7 @@ cudaError_t launch_synth_fill(uint64_t seed, uint64_t blob, uint64_t byte_off, v
     size_t blocks = (len / 16 + 255) / 256;
     clear_stale_error();
     if (blocks < 1) blocks = 1;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > kSms * 16) blocks = kSms * 16;
     synth_fill_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dm_blob_key(seed, blob), byte_off,
                                                             static_cast<uint8_t *>(dst), len);
     return cudaGetLastError();
@@ -949,7 +950,7 @@ cudaError_t launch_synth_fill_many(uint64_t seed, uint64_t first_blob, void *bas
     uint64_t blocks = (span / 16 + 255) / 256;
     clear_stale_error();
     if (blocks < 1) blocks = 1;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > kSms * 16) blocks = kSms * 16;
     synth_fill_many_kernel<<<(unsigned)blocks, 256, 0, stream>>>(seed, first_blob, static_cast<uint8_t *>(base),
                                                                  dev_offsets, dev_lengths, n, first_off, span);
     return cudaGetLastError();

@@ -1,4 +1,4 @@
-// Internal interface between the engine (host C++) and the sm_100a kernels.
+// Internal interface between the engine (host C++) and the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -36,27 +36,28 @@ cudaError_t launch_sha256_wide(const HashJob *jobs, uint32_t njobs, uint32_t *st
                                uint32_t *digests, cudaStream_t stream, int variant);
 cudaError_t launch_sha256_deep(const HashJob *jobs, uint32_t njobs, uint32_t *states,
                                uint32_t *digests, cudaStream_t stream, int variant);
-// fma 1 + style 5: rolled rounds, additions on the FMA pipe, every lane's next 128-byte line staged by cp.async in its own
-// shared-memory row.  Measured on B200, 151 552 streams x 112 KiB: style 2 (variant 9, round 1) 18.25 ms, style 5 17.07 ms.
-constexpr int kDefaultWideVariant = 21;
+// fma 1 + style 2: rolled rounds, additions on the FMA pipe, each lane's 128-byte line loaded into registers.  Measured
+// on H100 SXM, 135 168 streams x 112 KiB per launch: variant 9 25.2 ms, variant 21 (style 5: the next line staged in
+// shared memory by cp.async) 40.4 ms.
+constexpr int kDefaultWideVariant = 9;
 // S streams per warp, S in {2,4,8,16}: the middle ground between deep and wide.  `variant` is the deep
 // kernel's (the serial phase is the same code): 4..7 = the short-chain rounds, anything else = ptxas' ordering.
 cudaError_t launch_sha256_group(const HashJob *jobs, uint32_t njobs, uint32_t *states,
                                 uint32_t *digests, cudaStream_t stream, int streams_per_warp, int variant);
 
 // Kernel choice by live-stream count (DESIGN.md §5): aim for one to two warps on
-// each of the 592 sub-partitions.  Returns streams per warp: 1 = deep, 32 = wide.
-constexpr uint32_t kSubPartitions = 592;             // 148 SMs x 4
+// each of the 528 sub-partitions.  Returns streams per warp: 1 = deep, 32 = wide.
+constexpr uint32_t kSms = 132;                       // H100 SXM
+constexpr uint32_t kSubPartitions = kSms * 4;
 constexpr uint32_t kMaxWarpPairs = kSubPartitions / 2;
 
 inline int streams_per_warp_for(uint32_t njobs)
 {
-    // Measured on B200 (profiles/r02_streams_per_warp_sweep.txt): a warp must never share its sub-partition with
-    // another round warp (640 streams, one warp each: 340 ms; two per warp: 206 ms), and while there are sub-partitions
-    // to spare a SECOND warp per group - loading and expanding the next blocks' schedules ahead of the round warp -
-    // is worth far more than a smaller S (4096 streams: 16 per warp, paired: 30.7 ms; 16 per warp, alone: 41.8 ms).
-    // So: the smallest S in {1, 2, 4, 8, 16} whose njobs / S groups can each have a warp PAIR (<= 296 groups, up to
-    // 4736 streams); then 16 per warp, one warp per sub-partition (<= 9472 streams); then a lane per stream.
+    // A warp must never share its sub-partition with another round warp (the round chain is issue-bound on one
+    // sub-partition's ALU pipe), and while there are sub-partitions to spare a SECOND warp per group - loading and
+    // expanding the next blocks' schedules ahead of the round warp - is worth more than a smaller S (DESIGN.md §5).
+    // So: the smallest S in {1, 2, 4, 8, 16} whose njobs / S groups can each have a warp PAIR (<= 264 groups, up to
+    // 4224 streams); then 16 per warp, one warp per sub-partition (<= 8448 streams); then a lane per stream.
     for (int s = 1; s <= 16; s *= 2)
         if ((njobs + s - 1) / s <= kMaxWarpPairs) return s;
     if ((njobs + 15) / 16 <= kSubPartitions) return 16;
@@ -74,12 +75,11 @@ inline int streams_per_warp_unpaired(uint32_t njobs)
 // ones still running, all at S per warp) share the chip?
 inline bool warp_pairs_fit(uint32_t resident, int s) { return s <= 16 && (resident + (uint32_t)s - 1) / (uint32_t)s <= kMaxWarpPairs; }
 
-// Round form 7 = short-chain round with e' on the FMA pipe and a' as one IADD3 (sha256_round.cuh): measured on B200,
-// 256 x 8 MiB: variant 0 132.2 ms, 4 120.6, 5 119.1, 6 119.5, 7 110.7 (profiles/r02_round_variants.txt).
-// 8 = form 7 with TWO warps per stream while there are at most 296 jobs in the launch (a schedule warp runs ahead of
-// the round warp, sha256_deep2_kernel): 105.4 ms; larger launches fall back to 7 by themselves.
-// 9 = 8 plus the same split in the S-streams-per-warp kernels (sha256_group2_kernel) while the launch has at most 296
-// groups: 4096 streams 41.8 -> 30.7 ms, 2048 streams 75.5 -> 57.2 ms, 1024 streams 129.2 -> 111.0 ms.
+// Round form 7 = short-chain round with e' on the FMA pipe and a' as one IADD3 (sha256_round.cuh).
+// 8 = form 7 with TWO warps per stream while there are at most kMaxWarpPairs (264) jobs in the launch (a schedule
+// warp runs ahead of the round warp, sha256_deep2_kernel); larger launches fall back to 7 by themselves.
+// 9 = 8 plus the same split in the S-streams-per-warp kernels (sha256_group2_kernel) while the launch has at most
+// kMaxWarpPairs groups.
 constexpr int kDefaultDeepVariant = 9;
 
 

@@ -1,7 +1,7 @@
 """Python mirror of the C-ABI, used by tests and bench.py.
 
 Method names follow the hook-side vocabulary of the reference
-(/root/reference/cmd/demodel/start.go:197-204): a response body is *teed*
+(demodel/cmd/demodel/start.go:197-204): a response body is *teed*
 into a stream (open / write / finish / abort) and a request is answered from
 the cache (open / read / close).  All compute happens inside
 libdemodel_b200.so; nothing here hashes or copies blob bytes on the CPU.

@@ -2,7 +2,7 @@
 dm_manifest_parse / dm_manifest_prefetch.
 
 An Ollama / OCI pull fetches the image manifest first (shape: the reference's
-cached fixture, /root/reference/CONTRIBUTING.md:128-153); every layer's digest
+cached fixture, demodel/CONTRIBUTING.md:128-153); every layer's digest
 and size is known from it, so the proxy can reserve and verify each layer
 stream before its body arrives.
 """

@@ -1,9 +1,9 @@
 /*
- * demodel_b200.h — C-ABI of the B200 blob hash-and-cache engine.
+ * demodel_b200.h — C-ABI of the H100 blob hash-and-cache engine.
  *
  * This is the drop-in boundary for demodel's cache path.  The reference
  * (moeru-ai/demodel @ fb8342aa) has no FFI, plugin or C interface of its own
- * (SURVEY.md §8b; /root/reference/pkg/utils/fs.go:1-8 is all of pkg/), so
+ * (SURVEY.md §8b; demodel/pkg/utils/fs.go:1-8 is all of pkg/), so
  * each entry point below cites the reference *hook* whose body it serves:
  *
  *   OnResponse hook  cmd/demodel/start.go:201-204   (today: Println, return resp)
@@ -222,7 +222,7 @@ int dm_cache_follow(dm_engine *e, const uint8_t digest[32], uint64_t *reader, ui
 
 /* URL -> digest index for the OnRequest hit check (start.go:197-200 hands the hook a request, not a
  * digest).  OCI blob URLs carry `sha256:<hex>`; HuggingFace `resolve/<rev>/<file>` URLs (the first clients
- * /root/reference/README.md:16-21 lists) do not.  The tee records URL (or ETag / LFS oid string) -> digest
+ * demodel/README.md:16-21 lists) do not.  The tee records URL (or ETag / LFS oid string) -> digest
  * when a body verifies; a later request for the same key is answered from the CAS.  `key` is any
  * NUL-terminated string up to 4096 bytes.  With cas_dir the index is an append-only log
  * (<cas_dir>/aliases.log) replayed by dm_engine_create; a put for an existing key replaces it.

@@ -4,7 +4,7 @@
  * The CPU arm of the benchmark: the hash-and-cache loop north_star attributes
  * to the reference ("Go io.Copy + crypto/sha256"), restated for this image.
  * The reference holds no such loop (SURVEY.md §0: the hooks at
- * /root/reference/cmd/demodel/start.go:197-204 only print) and Go is not
+ * demodel/cmd/demodel/start.go:197-204 only print) and Go is not
  * installed, so the stand-in is what that loop would be:
  *
  *     for each blob (one goroutine per connection -> one thread per blob):

@@ -6,9 +6,9 @@
  * --impl reference legs may load this; nothing under demodel_b200/ does.
  *
  * What it restates.  BASELINE.json's north_star names Go's standard-library
- * crypto/sha256 (Go 1.24.3 per /root/reference/go.mod:3) as the reference
+ * crypto/sha256 (Go 1.24.3 per demodel/go.mod:3) as the reference
  * digest.  The reference repository itself has NO call site of it — the
- * response hook at /root/reference/cmd/demodel/start.go:201-204 only prints
+ * response hook at demodel/cmd/demodel/start.go:201-204 only prints
  * and returns resp unchanged, and grep finds no sha256 import (SURVEY.md §0).
  * crypto/sha256 is an implementation of FIPS 180-4 SHA-256, so this file
  * restates FIPS 180-4 §4.1.2 (functions), §4.2.2 (constants), §5.1.1

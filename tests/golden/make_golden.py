@@ -1,11 +1,12 @@
 #!/usr/bin/env python3
 """Regenerates tests/golden/*.json from sources that exist in THIS container.
 
-Run here (the GPU box has no /root/reference):  python tests/golden/make_golden.py
+Run from a checkout of the reference:  python tests/golden/make_golden.py <path to moeru-ai/demodel checkout>
+(without the path only fips_vectors.json is rewritten)
 
 1. reference_fixture.json — the only byte-level fixture the reference ships:
    the xxd dump of a cached, gzip-encoded Ollama manifest body at
-   /root/reference/CONTRIBUTING.md:76-99, plus the manifest JSON it inflates
+   demodel/CONTRIBUTING.md:76-99, plus the manifest JSON it inflates
    to (CONTRIBUTING.md:128-153).  The reference states no digest for either;
    the digests recorded here are hashlib's (cross-checked against OpenSSL by
    tests/test_oracle.py).
@@ -18,9 +19,10 @@ import hashlib
 import json
 import os
 import re
+import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/CONTRIBUTING.md"
+REF = os.path.join(sys.argv[1], "CONTRIBUTING.md") if len(sys.argv) > 1 else None
 
 
 def reference_fixture():
@@ -86,11 +88,11 @@ def fips_vectors():
 def main():
     with open(os.path.join(HERE, "fips_vectors.json"), "w") as f:
         json.dump(fips_vectors(), f, indent=1)
-    if os.path.exists(REF):
+    if REF and os.path.exists(REF):
         with open(os.path.join(HERE, "reference_fixture.json"), "w") as f:
             json.dump(reference_fixture(), f, indent=1)
     else:
-        print("no /root/reference here: reference_fixture.json left as committed")
+        print("no reference checkout given: reference_fixture.json left as committed")
 
 
 if __name__ == "__main__":

@@ -16,7 +16,7 @@ _lib.LIB_PATH = sys.argv[1]
 import numpy as np  # noqa: E402
 import demodel_b200  # noqa: E402
 
-n = int(sys.argv[2]) if len(sys.argv) > 2 else 151552
+n = int(sys.argv[2]) if len(sys.argv) > 2 else 135168
 steps = int(sys.argv[3]) if len(sys.argv) > 3 else 5
 size = 256
 host = np.zeros(n * size, dtype=np.uint8)             # "device" memory of the fake runtime is host memory

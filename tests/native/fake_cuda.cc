@@ -111,7 +111,7 @@ static void on_stream(cudaStream_t s, std::function<void()> f)
 extern "C" {
 cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 cudaError_t cudaSetDevice(int) { return cudaSuccess; }
-cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { memset(p, 0, sizeof *p); p->major = 10; p->multiProcessorCount = 148; return cudaSuccess; }
+cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { memset(p, 0, sizeof *p); p->major = 9; p->minor = 0; p->multiProcessorCount = 132; return cudaSuccess; }
 cudaError_t cudaDeviceSynchronize(void)
 {
     std::vector<fakeStream *> all;

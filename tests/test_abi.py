@@ -114,7 +114,7 @@ def test_reference_arm_runs_without_a_gpu():
 
 def test_kernel_selection_rule_and_bench_mirror():
     """streams_per_warp_for(): monotone, powers of two; while there are sub-partitions to spare every group of S streams
-    gets a warp PAIR (at most 296 groups, so up to 4736 streams), then one warp per sub-partition (592) at S = 16, then
+    gets a warp PAIR (at most 264 groups, so up to 4224 streams), then one warp per sub-partition (528) at S = 16, then
     a lane per stream - deep (S = 1, paired) for the BASELINE 256-stream config; bench.py's report label mirrors it."""
     import importlib.util
     lib = demodel_b200.load()
@@ -122,22 +122,22 @@ def test_kernel_selection_rule_and_bench_mirror():
     bench = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(bench)
     prev = 0
-    edges = [296, 297, 592, 593, 1184, 1185, 2368, 2369, 4736, 4737, 9472, 9473]
-    for n in list(range(1, 20000, 37)) + [256, 151552, 1 << 31] + edges:
+    edges = [264, 265, 528, 529, 1056, 1057, 2112, 2113, 4224, 4225, 8448, 8449]
+    for n in list(range(1, 20000, 37)) + [256, 135168, 1 << 31] + edges:
         spw = lib.dm_streams_per_warp(n)
         assert spw in (1, 2, 4, 8, 16, 32)
         groups = (n + spw - 1) // spw
-        assert spw == 32 or groups <= 592
-        assert spw in (16, 32) or groups <= 296                         # S < 16 is only ever chosen with room for pairs
+        assert spw == 32 or groups <= 528
+        assert spw in (16, 32) or groups <= 264                         # S < 16 is only ever chosen with room for pairs
         label = bench._kernel_for(n)
-        assert (f"{spw} stream" in label) and (("pair" in label) == (spw < 32 and groups <= 296))
+        assert (f"{spw} stream" in label) and (("pair" in label) == (spw < 32 and groups <= 264))
     for n in sorted(list(range(1, 20000, 37)) + edges):
         spw = lib.dm_streams_per_warp(n)
         assert spw >= prev
         prev = spw
-    assert lib.dm_streams_per_warp(256) == 1 and lib.dm_streams_per_warp(9473) == 32 and lib.dm_streams_per_warp(4096) == 16
-    assert lib.dm_streams_per_warp(296) == 1 and lib.dm_streams_per_warp(297) == 2 and lib.dm_streams_per_warp(592) == 2
-    assert lib.dm_streams_per_warp(593) == 4 and lib.dm_streams_per_warp(6144) == 16 and lib.dm_streams_per_warp(4737) == 16
+    assert lib.dm_streams_per_warp(256) == 1 and lib.dm_streams_per_warp(8449) == 32 and lib.dm_streams_per_warp(4096) == 16
+    assert lib.dm_streams_per_warp(264) == 1 and lib.dm_streams_per_warp(265) == 2 and lib.dm_streams_per_warp(528) == 2
+    assert lib.dm_streams_per_warp(529) == 4 and lib.dm_streams_per_warp(6144) == 16 and lib.dm_streams_per_warp(4225) == 16
 
 
 def test_bench_rank_partition_is_disjoint_and_complete():

@@ -1,7 +1,7 @@
 """Every selectable round ordering (DM_KERNEL_VARIANT) is bit-exact on the GPU, not only the default.
 
 Each runs in a process of its own (the variant is read once, at engine creation).  The default deep variant
-(8: round form 7, two warps per stream in launches of at most 296 jobs) is what tests/test_gpu_parity.py exercises on every kernel shape; here the alternatives that stay
+(8: round form 7, two warps per stream in launches of at most 264 jobs) is what tests/test_gpu_parity.py exercises on every kernel shape; here the alternatives that stay
 selectable for A/B runs - ptxas' own ordering (0), the other short-chain forms (4, 5) and the wide kernel with
 cp.async-staged lines (21) - are held to the
 same bar by tools/check_variant.py: every length 0..300, group / line boundaries, 1500 ragged blobs in one

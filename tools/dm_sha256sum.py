@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""sha256sum-compatible digest of files, computed by the B200 engine (one stream per file, all
+"""sha256sum-compatible digest of files, computed by the GPU engine (one stream per file, all
 files in flight together so the multi-buffer kernel has something to batch).
 
     python tools/dm_sha256sum.py [--device 0] [--check SUMS] FILE...

@@ -3,8 +3,8 @@
 
 For the single-warp serial phase of the deep kernel (one warp per stream, alone on
 its sub-partition) nothing hides latency, so the cycles per round can be estimated
-from the SASS alone.  Model (numbers from /opt/skills/guides/B300_MICROARCH.md
-"Pipe rates & latencies" and profiles/r01_ubench_issue_rates.txt):
+from the SASS alone.  Model (pipe rates and latencies as tools/ubench/pipemix.cu and
+chainlat.cu measure them):
 
   * in-order issue, at most one instruction per cycle;
   * the ALU pipe (SHF, LOP3, IADD3, PRMT, VIADD, ISETP, MOV ...) and the FMA pipe
@@ -19,9 +19,9 @@ Usage:
 Picks the loop between the first and last LDS of the named function (the phase-2
 block loop), replays it `iters` times and prints cycles per iteration in steady
 state, the pipe-issue lower bounds and the critical-path bound.  It is a ranking
-tool for candidate round orderings when no GPU is at hand; calibration against the
-one measured point (deep<0>: ~1880 cycles per block in phase 2, 16.57 ms per
-256 x 1 MiB launch at 1.9 GHz) is printed by --calibrate.
+tool for candidate round orderings when no GPU is at hand.  On an H100 SXM the
+model reads 35.0 cycles per round for deep<0> and 24.3 for deep<7>; measured at
+1.98 GHz (256 x 1 MiB per launch) they take 37.8 and 26.5.
 """
 import argparse
 import re

@@ -5,7 +5,7 @@ For a single in-order warp running fixed-latency integer code (the deep / group 
 issue time of the loop is, to first order, the sum over its instructions of the `stall` field ptxas encoded
 (bits 105..108 of each 128-bit instruction: cycles to wait before issuing the next one) - ncu shows exactly
 that for the shipped kernel: `selected` 1.00 + `wait` 1.02 per issue and nothing else
-(profiles/r01_ncu_deep_shipped_metrics.csv).  Comparing this number with the measured launch time says whether
+(ncu metrics of the deep kernel).  Comparing this number with the measured launch time says whether
 a form is limited by ptxas' own schedule or by something the hardware adds on top.
 
   cuobjdump -sass build/sha256_kernels.o > all.sass; tools/sass_stalls.py all.sass 'deep_kernelILi7E'
@@ -53,7 +53,7 @@ def main():
     rounds = max(16, 16 * round(ops["SHF"] / 96))     # 6 rotations per round (+ a few address shifts): 64 (unrolled) or 16 (rolled) rounds per iteration
     print(f"{sys.argv[2]}: {len(loop)} instructions in the loop ({rounds} rounds per iteration): " + ", ".join(f"{k} {v}" for k, v in ops.most_common(8)))
     print(f"  sum of ptxas stall counts = {total} cycles per iteration = {total / rounds:.2f} cycles per round"
-          f" -> {1.965e9 / (total / rounds) / 1e6:.1f} MB/s per stream at 1.965 GHz (phase 2 only)")
+          f" -> {1.98e9 / (total / rounds) / 1e6:.1f} MB/s per stream at 1.98 GHz (phase 2 only)")
 
 
 if __name__ == "__main__":

@@ -3,7 +3,7 @@
 //   dependent chains:  SHF->SHF, IMAD->IMAD, SHF->IMAD->SHF (cross-pipe), IMAD.WIDE, IMAD.HI
 //   independent x4:    IMAD with an immediate multiplier (is the imm form 1/cycle like FFMA-imm?),
 //                      IMAD.WIDE, IMAD.HI   (are they full rate on the FMA pipe?)
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o chainlat chainlat.cu && ./chainlat
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o chainlat chainlat.cu && ./chainlat
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -35,7 +35,7 @@ template <int MODE> void run(const char *name, unsigned *out)
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     const int iters = 20000;
     for (int wps : {1, 2, 4}) {                 // warps per sub-partition (4 sub-partitions per SM)
-        const int blocks = 148 * 4 * wps;
+        const int blocks = 132 * 4 * wps;        // H100 SXM: 132 SMs
         chain<MODE><<<blocks, 32>>>(out, 100, 1u);
         cudaDeviceSynchronize();
         cudaEventRecord(e0);
@@ -44,13 +44,13 @@ template <int MODE> void run(const char *name, unsigned *out)
         cudaEventSynchronize(e1);
         float ms; cudaEventElapsedTime(&ms, e0, e1);
         printf("%-22s warps/sub-partition=%d  %.2f cycles per 4-instruction group per warp\n", name, wps,
-               ms * 1e-3 * 1.965e9 / ((double)iters * 32));
+               ms * 1e-3 * 1.98e9 / ((double)iters * 32));
     }
 }
 int main()
 {
     unsigned *out;
-    cudaMalloc(&out, 4 * 32 * 148 * 16);
+    cudaMalloc(&out, 4 * 32 * 132 * 16);
     run<0>("4 ALU (SHF,SHF,LOP3,LOP3)", out);
     run<1>("4 IMAD", out);
     run<2>("2 ALU + 2 IMAD", out);
