@@ -641,7 +641,7 @@ static int ingest_device_impl(dm_engine *e, const void *dev_base, const uint64_t
     // the two launches of a split batch share the chip: the rest runs one warp per group (the long jobs keep their
     // warp pairs while there are at most kMaxWarpPairs of them)
     const int spw_rest = n_long ? dm::streams_per_warp_unpaired(n_rest) : spw;
-    const int v_rest = n_long && e->variant_deep >= 8 ? 7 : e->variant_deep;
+    const dm::KernelShape rest_shape = dm::kernel_shape(spw_rest, n_long ? 0 : n, e->variant_wide, e->variant_deep);
     // Very large lane-per-stream batches go out in chunks, each on a stream of its own: at 10^5 blobs the host work
     // around the launch (extents, index) is of the order of the kernel itself, and this way all but the first
     // chunk's preparation and the last chunk's publication happens while kernels run.  The launches overlap on the
@@ -675,7 +675,7 @@ static int ingest_device_impl(dm_engine *e, const void *dev_base, const uint64_t
             cudaStream_t cs = e->ing_streams[c];
             err = cudaMemcpyAsync(e->ing_jobs_d + lo, e->ing_jobs_h + lo, sizeof(dm::HashJob) * (uint64_t)(hi - lo), cudaMemcpyHostToDevice, cs);
             if (err == cudaSuccess && c == 0) err = cudaEventRecord(e->ing_ev0, cs);
-            if (err == cudaSuccess) err = dm::launch_sha256_wide(e->ing_jobs_d + lo, hi - lo, e->ing_states, e->ing_digests, cs, e->variant_wide);
+            if (err == cudaSuccess) err = dm::launch_sha256(e->ing_jobs_d + lo, hi - lo, e->ing_states, e->ing_digests, cs, rest_shape);
             if (err == cudaSuccess) err = cudaEventRecord(e->ing_cev_k[c], cs);
             if (err == cudaSuccess) err = cudaMemcpyAsync(e->ing_digests_h + 8ull * lo, e->ing_digests + 8ull * lo, 32ull * (hi - lo), cudaMemcpyDeviceToHost, cs);
             if (err == cudaSuccess) err = cudaEventRecord(e->ing_cev_done[c], cs);
@@ -707,15 +707,12 @@ static int ingest_device_impl(dm_engine *e, const void *dev_base, const uint64_t
         if (err == cudaSuccess) err = cudaEventRecord(e->ing_ev0, st);
         if (err == cudaSuccess && n_long) {
             err = cudaStreamWaitEvent(st2, e->ing_ev0, 0);              // the job table is in place
-            if (err == cudaSuccess) err = dm::launch_sha256_deep(e->ing_jobs_d, n_long, e->ing_states, e->ing_digests, st2, e->variant_deep);
+            if (err == cudaSuccess)
+                err = dm::launch_sha256(e->ing_jobs_d, n_long, e->ing_states, e->ing_digests, st2,
+                                        dm::kernel_shape(1, n_long, e->variant_wide, e->variant_deep));
             if (err == cudaSuccess) err = cudaEventRecord(e->ing_ev2, st2);
         }
-        if (err == cudaSuccess) {
-            const dm::HashJob *rest = e->ing_jobs_d + n_long;
-            err = spw_rest == 1 ? dm::launch_sha256_deep(rest, n_rest, e->ing_states, e->ing_digests, st, v_rest)
-                : spw_rest == 32 ? dm::launch_sha256_wide(rest, n_rest, e->ing_states, e->ing_digests, st, e->variant_wide)
-                                 : dm::launch_sha256_group(rest, n_rest, e->ing_states, e->ing_digests, st, spw_rest, v_rest);
-        }
+        if (err == cudaSuccess) err = dm::launch_sha256(e->ing_jobs_d + n_long, n_rest, e->ing_states, e->ing_digests, st, rest_shape);
         if (err == cudaSuccess) err = cudaEventRecord(e->ing_ev1, st);
         if (err == cudaSuccess && n_long) err = cudaStreamWaitEvent(st, e->ing_ev2, 0);       // digests of both launches
         if (err == cudaSuccess) err = cudaMemcpyAsync(e->ing_digests_h, e->ing_digests, 32ull * n, cudaMemcpyDeviceToHost, st);

@@ -852,9 +852,9 @@ bool run_cycle(dm_engine *e, Cycle &c, std::vector<std::shared_ptr<Stream>> &rea
     for (const Cycle &o : e->cycles) if (o.busy) resident += o.njobs;
     const int spw = e->force_spw ? e->force_spw : dm::streams_per_warp_for(resident);
     c.deep = spw == 1;
-    // warp pairs (variants 8 / 9) only while ALL co-resident groups can have two sub-partitions each: a round warp
-    // that shares its sub-partition with another one runs at half speed
-    const int deep_variant = (e->variant_deep >= 8 && !dm::warp_pairs_fit(resident, spw)) ? 7 : e->variant_deep;
+    // warp pairs only while ALL co-resident groups can have two sub-partitions each: a round warp that shares its
+    // sub-partition with another one runs at half speed
+    const dm::KernelShape shape = dm::kernel_shape(spw, resident, e->variant_wide, e->variant_deep);
     if (spw > 1) {
         // lanes of a warp run in lock step: keep neighbours the same length
         std::vector<uint32_t> order(c.njobs);
@@ -879,9 +879,10 @@ bool run_cycle(dm_engine *e, Cycle &c, std::vector<std::shared_ptr<Stream>> &rea
     note(cudaMemcpyAsync(c.d_jobs, c.h_jobs, sizeof(dm::HashJob) * c.njobs, cudaMemcpyHostToDevice, c.stream));
     note(cudaEventRecord(c.k_start, c.stream));
     if (c.err != cudaSuccess) { /* the job table may not be on the device: launching would run stale jobs */ }
-    else if (spw == 1) { note(dm::launch_sha256_deep(c.d_jobs, c.njobs, e->d_states, e->d_digests, c.stream, deep_variant)); e->st_deep++; }
-    else if (spw == 32) { note(dm::launch_sha256_wide(c.d_jobs, c.njobs, e->d_states, e->d_digests, c.stream, e->variant_wide)); e->st_wide++; }
-    else { note(dm::launch_sha256_group(c.d_jobs, c.njobs, e->d_states, e->d_digests, c.stream, spw, deep_variant)); e->st_group++; }
+    else {
+        note(dm::launch_sha256(c.d_jobs, c.njobs, e->d_states, e->d_digests, c.stream, shape));
+        (spw == 1 ? e->st_deep : spw == 32 ? e->st_wide : e->st_group)++;
+    }
     e->st_launches++;
     note(cudaEventRecord(c.k_end, c.stream));
     c.busy = true;

@@ -1,8 +1,8 @@
 // Multi-buffer SHA-256 for sm_90a (H100): the hot path of the blob hash-and-cache
 // engine.  Pure 32-bit integer work (SHF / LOP3 / IADD3 / IMAD) — no tensor
-// cores, no floating point.  Three kernel shapes share the round function;
-// the engine picks one per launch from the number of co-resident streams
-// (streams_per_warp_for):
+// cores, no floating point.  Two kernels share the round function; the
+// engine picks a shape per launch from the number of co-resident streams
+// (streams_per_warp_for, kernel_shape):
 //
 //   sha256_wide_kernel   one 32-bit lane per live stream (the multi-buffer
 //                        form north_star describes): W[16] and the eight
@@ -17,19 +17,16 @@
 //                        pipe (one warp-instruction per 2 cycles per
 //                        sub-partition): <= ~1.0 TB/s on 132 SMs at 1.98 GHz;
 //                        needs > ~10^4 streams to fill the chip.
-//   sha256_deep_kernel   one warp per stream, for few live streams.  SHA-256's
-//                        serial chain is only the 64 rounds; the message
-//                        schedule is state-independent.  The 32 lanes expand
-//                        the schedules of 32 consecutive blocks in parallel
-//                        (coalesced 2 KiB load) and stage W[t]+K[t] in shared
-//                        memory; then the warp runs the 32x64 dependent rounds
-//                        reading one broadcast LDS.128 per 4 rounds.  ~1.9x the
-//                        per-stream rate of the lane-per-stream form.
-//   sha256_group_kernel  S = 2/4/8/16 streams per warp: the deep kernel's two
-//                        phases with lane = block_slot * S + stream, so S round
-//                        chains advance per instruction.  Wins between 265 and
-//                        ~8 500 streams (S = the smallest that keeps one warp per
-//                        sub-partition).
+//   sha256_warp_kernel   S = 1/2/4/8/16 streams per warp, for fewer live
+//                        streams.  SHA-256's serial chain is only the 64
+//                        rounds; the message schedule is state-independent.
+//                        The 32 lanes expand the schedules of 32 blocks in
+//                        parallel (lane = block_slot * S + stream, coalesced
+//                        loads) and stage W[t]+K[t] in shared memory; then the
+//                        warp runs 32/S block-steps of 64 dependent rounds, S
+//                        round chains per instruction, reading one broadcast
+//                        LDS.128 per 4 rounds.  As a warp pair, a second warp
+//                        does the loads and schedules one group ahead.
 //
 // All optionally write every byte they read to `dst` (the blob's CAS
 // extent), so hash-and-cache moves 1 B read + 1 B written per blob byte;
@@ -366,9 +363,23 @@ sha256_wide_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *_
     store_state(s, states, digests, jb.slot, jb.flags);
 }
 
-// Phase 1 of the deep and group kernels: one lane expands the 64-entry schedule of its block and
-// stages W[t] + K[t] as 16 uint4 (FIPS 180-4 §6.2.2 step 1, K folded in).  Additions are left to ptxas:
-// forcing them onto the FMA pipe lengthens the w[t-2] -> w[t] chain and the timing model shows no gain.
+// ---------------------------------------------------------------------------
+// warp: S = 1, 2, 4, 8 or 16 streams per warp, optionally as a warp pair
+// ---------------------------------------------------------------------------
+// Two phases per group of 32 blocks.  Phase 1: the warp's 32 lanes, lane = b * S + j (stream j, block slot b, B = 32 / S
+// blocks per stream), each load one block, write its CAS copy and stage that block's 64-entry schedule, K folded in, as
+// a row of shared memory.  Phase 2: B dependent block-steps of 64 rounds, every lane following stream j and reading one
+// broadcast LDS.128 per 4 rounds, so S round chains advance per instruction.  Lanes with the same j compute identical
+// values (no divergence); a row read is S distinct 16-byte words per LDS.128 (conflict-free for S <= 8, two-way for
+// S = 16).  Streams in a warp may differ in length: a lane stops updating its state when its stream has no block in
+// a step.  S = 1 (one warp per stream) is ~1.9x the per-stream rate of the lane-per-stream form.
+constexpr int kKwStride = 68;                 // words per staged block: 64 + 4 pad -> conflict-free STS.128
+constexpr int kWarpsPerCta = 1;               // one-warp form; 1 lets the block scheduler spread few streams over
+                                              // all 528 sub-partitions
+
+// One lane expands the 64-entry schedule of its block and stages W[t] + K[t] as 16 uint4 (FIPS 180-4 §6.2.2 step 1,
+// K folded in).  Additions are left to ptxas: forcing them onto the FMA pipe lengthens the w[t-2] -> w[t] chain and
+// the timing model shows no gain.
 __device__ __forceinline__ void expand_schedule(uint32_t (&w)[16], uint4 *out)
 {
     constexpr uint32_t K[64] = {DM_K256_TABLE};
@@ -385,98 +396,63 @@ __device__ __forceinline__ void expand_schedule(uint32_t (&w)[16], uint4 *out)
     }
 }
 
-// ---------------------------------------------------------------------------
-// deep: one warp per stream
-// ---------------------------------------------------------------------------
-constexpr int kDeepWarps = 1;                 // warps per CTA; 1 lets the block scheduler
-                                              // spread few streams over all 528 sub-partitions
-constexpr int kKwStride = 68;                 // words per staged block: 64 + 4 pad -> conflict-free STS.128
-
-template <int kFma>
-__global__ void __launch_bounds__(32 * kDeepWarps)
-sha256_deep_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *__restrict__ states,
-                   uint32_t *__restrict__ digests, FmaK k)
+// Phase 1 of group g for one lane (block slot b = lane / S): if its stream has that block (held in x), copy it out and
+// stage its schedule in `row`; then load the lane's block of the next group.  kSync: this warp reads the rows itself,
+// so they are published (__syncwarp) first.  The order of the steps and the 32-bit in-group tests at S = 1 are what
+// ptxas schedules the rounds best after (tools/sass_sched.py); at S > 1 a stream may have run out before group g.
+template <int S, bool kSync>
+__device__ __forceinline__ void stage_block(uint4 (&x)[4], const uint4 *&p, uint4 *&q, bool copy, uint32_t lane,
+                                            uint64_t g, uint64_t ngroups, uint64_t nblk, uint4 *row)
 {
-    __shared__ __align__(16) uint32_t kw_smem[kDeepWarps][32 * kKwStride];
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t wid = threadIdx.x >> 5;
-    const uint32_t j = blockIdx.x * kDeepWarps + wid;
-    if (j >= njobs) return;
-    const HashJob jb = load_job(jobs, j);
-    uint32_t s[8];
-    load_state(s, states, jb.slot, jb.flags);
-    uint32_t *kw = kw_smem[wid];
-    if constexpr (kFma == 2) k.one = jb.one;
-
-    const uint64_t nblk = jb.nbytes >> 6;
-    const uint64_t ngroups = (nblk + 31) >> 5;
-    const bool copy = jb.dst != nullptr;
-    const uint4 *p = reinterpret_cast<const uint4 *>(jb.src) + 4ull * lane;   // this lane's block in group 0
-    uint4 *q = reinterpret_cast<uint4 *>(jb.dst) + 4ull * lane;
-
-    uint4 x[4];
-    if (lane < nblk) {
+    constexpr uint32_t B = 32 / S;
+    const uint32_t b = lane / S;
+    const uint64_t blk0 = g * B, left = nblk - blk0;
+    if (S == 1 ? lane < (left < 32 ? (uint32_t)left : 32u) : blk0 + b < nblk) {
+        if (copy) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) st_stream(q + i, x[i]);
+        }
+        uint32_t w[16];
+        unpack_be(w, x[0], x[1], x[2], x[3]);
+        expand_schedule(w, row);
+    }
+    if constexpr (kSync) __syncwarp();
+    p += 4 * B; q += 4 * B;
+    if (S == 1 ? g + 1 < ngroups && lane < left - 32 : blk0 + B + b < nblk) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
     }
-#pragma unroll 1
-    for (uint64_t g = 0; g < ngroups; ++g) {
-        const uint64_t left = nblk - (g << 5);
-        const uint32_t nv = left < 32 ? (uint32_t)left : 32u;
-        // phase 1: every lane expands the schedule of its own block, K folded in
-        if (lane < nv) {
-            if (copy) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) st_stream(q + i, x[i]);
-            }
-            uint32_t w[16];
-            unpack_be(w, x[0], x[1], x[2], x[3]);
-            uint4 *out = reinterpret_cast<uint4 *>(kw + lane * kKwStride);
-            expand_schedule(w, out);
-        }
-        __syncwarp();
-        // prefetch the next group's block while the serial rounds run
-        p += 128; q += 128;
-        if (g + 1 < ngroups && lane < left - 32) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
-        }
-        // phase 2: the dependent chain, warp-uniform, one broadcast LDS.128 per 4 rounds
-#pragma unroll 1
-        for (uint32_t b = 0; b < nv; ++b) {
-            const uint4 *kp = reinterpret_cast<const uint4 *>(kw + b * kKwStride);
-            uint32_t v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = s[i];
-            sha_rounds4<kFma, 0>(v, kp[0], k);   sha_rounds4<kFma, 4>(v, kp[1], k);
-            sha_rounds4<kFma, 8>(v, kp[2], k);   sha_rounds4<kFma, 12>(v, kp[3], k);
-            sha_rounds4<kFma, 16>(v, kp[4], k);  sha_rounds4<kFma, 20>(v, kp[5], k);
-            sha_rounds4<kFma, 24>(v, kp[6], k);  sha_rounds4<kFma, 28>(v, kp[7], k);
-            sha_rounds4<kFma, 32>(v, kp[8], k);  sha_rounds4<kFma, 36>(v, kp[9], k);
-            sha_rounds4<kFma, 40>(v, kp[10], k); sha_rounds4<kFma, 44>(v, kp[11], k);
-            sha_rounds4<kFma, 48>(v, kp[12], k); sha_rounds4<kFma, 52>(v, kp[13], k);
-            sha_rounds4<kFma, 56>(v, kp[14], k); sha_rounds4<kFma, 60>(v, kp[15], k);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) s[i] += v[i];
-        }
-        __syncwarp();
-    }
-    const uint64_t done = nblk << 6;
-    hash_tail<kFma>(s, jb.src + done, copy ? jb.dst + done : nullptr, (uint32_t)(jb.nbytes & 63u),
-                    (jb.flags & JOB_FINAL) != 0, jb.total_len, lane == 0, k);
-    if (lane == 0) store_state(s, states, digests, jb.slot, jb.flags);
 }
 
-// ---------------------------------------------------------------------------
-// deep2: two warps per stream - a schedule warp runs ahead of the round warp
-// ---------------------------------------------------------------------------
-// With at most 264 live streams (half the sub-partitions) every stream can have TWO warps, each on a sub-partition
-// of its own.  The serial chain stays what it is - 64 dependent rounds per block on one warp - but everything else
-// leaves that warp: warp 1 loads the next 32 blocks, stores the fused CAS copy and expands the 32 message
-// schedules into the other half of a double-buffered W+K stage while warp 0 is still running the rounds of the
-// current 32.  Hand-over by named barriers (FULL / EMPTY per buffer: one side arrives, the other waits); the round
-// warp never touches global memory inside the loop.  What it buys is phase 1's share of the deep kernel: ~1 cycle
-// per round of 25.9.
+// Phase 2, one block-step: the 64 dependent rounds on one staged row, then the feed-forward, kept only where the
+// lane's stream has a block in this step (`valid`, always true for one stream per warp).
+template <int kFma>
+__device__ __forceinline__ void block_step(uint32_t (&s)[8], const uint4 *kp, bool valid, const FmaK &k)
+{
+    uint32_t v[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = s[i];
+    sha_rounds4<kFma, 0>(v, kp[0], k);   sha_rounds4<kFma, 4>(v, kp[1], k);
+    sha_rounds4<kFma, 8>(v, kp[2], k);   sha_rounds4<kFma, 12>(v, kp[3], k);
+    sha_rounds4<kFma, 16>(v, kp[4], k);  sha_rounds4<kFma, 20>(v, kp[5], k);
+    sha_rounds4<kFma, 24>(v, kp[6], k);  sha_rounds4<kFma, 28>(v, kp[7], k);
+    sha_rounds4<kFma, 32>(v, kp[8], k);  sha_rounds4<kFma, 36>(v, kp[9], k);
+    sha_rounds4<kFma, 40>(v, kp[10], k); sha_rounds4<kFma, 44>(v, kp[11], k);
+    sha_rounds4<kFma, 48>(v, kp[12], k); sha_rounds4<kFma, 52>(v, kp[13], k);
+    sha_rounds4<kFma, 56>(v, kp[14], k); sha_rounds4<kFma, 60>(v, kp[15], k);
+    if (valid) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) s[i] += v[i];
+    }
+}
+
+// kPair: two warps per group of S streams, for launches where every group can have two sub-partitions.  The serial
+// chain stays on one warp (warp 0), but everything else leaves it: warp 1 loads the next group's blocks, stores the
+// fused CAS copy and expands the schedules into the other half of a double-buffered stage while warp 0 still runs the
+// rounds of the current group.  Hand-over by named barriers (FULL / EMPTY per buffer: one side arrives, the other
+// waits); the round warp never touches global memory inside the loop.  What it buys is phase 1's share of the
+// one-warp form: ~1 cycle per round of 25.9 at S = 1, but per group of 32 blocks phase 1 costs ~1500 cycles against
+// (32 / S) x ~1600 for the rounds - 19 % of the time at S = 8, 32 % at S = 16.
 // (barrier ids as immediates: with a register id ptxas reserves all 16 named barriers for the CTA, and the SM's
 //  barrier pool then limits how many CTAs can be resident)
 template <int kId> __device__ __forceinline__ void named_bar_sync() { asm volatile("barrier.sync %0, 64;" :: "n"(kId) : "memory"); }
@@ -486,282 +462,97 @@ __device__ __forceinline__ void full_arrive(uint32_t b) { if (b) named_bar_arriv
 __device__ __forceinline__ void empty_sync(uint32_t b) { if (b) named_bar_sync<4>(); else named_bar_sync<3>(); }
 __device__ __forceinline__ void empty_arrive(uint32_t b) { if (b) named_bar_arrive<4>(); else named_bar_arrive<3>(); }
 
-template <int kFma>
-__global__ void __launch_bounds__(64)
-sha256_deep2_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *__restrict__ states,
-                    uint32_t *__restrict__ digests, FmaK k)
-{
-    __shared__ __align__(16) uint32_t kw_smem[2][32 * kKwStride];
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t role = threadIdx.x >> 5;          // 0: rounds, 1: loads + schedules
-    const uint32_t j = blockIdx.x;
-    if (j >= njobs) return;
-    const HashJob jb = load_job(jobs, j);
-    const uint64_t nblk = jb.nbytes >> 6;
-    const uint64_t ngroups = (nblk + 31) >> 5;
-    const bool copy = jb.dst != nullptr;
-
-    if (role == 1) {
-        const uint4 *p = reinterpret_cast<const uint4 *>(jb.src) + 4ull * lane;
-        uint4 *q = reinterpret_cast<uint4 *>(jb.dst) + 4ull * lane;
-        uint4 x[4];
-        if (lane < nblk) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
-        }
-#pragma unroll 1
-        for (uint64_t g = 0; g < ngroups; ++g) {
-            const uint64_t left = nblk - (g << 5);
-            const uint32_t nv = left < 32 ? (uint32_t)left : 32u;
-            const uint32_t b = (uint32_t)g & 1u;
-            empty_sync(b);                                                // the round warp is done with this buffer
-            if (lane < nv) {
-                if (copy) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) st_stream(q + i, x[i]);
-                }
-                uint32_t w[16];
-                unpack_be(w, x[0], x[1], x[2], x[3]);
-                expand_schedule(w, reinterpret_cast<uint4 *>(kw_smem[b] + lane * kKwStride));
-            }
-            p += 128; q += 128;
-            if (g + 1 < ngroups && lane < left - 32) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
-            }
-            __threadfence_block();                                        // the stage is written before it is announced
-            full_arrive(b);
-        }
-        return;
-    }
-
-    uint32_t s[8];
-    load_state(s, states, jb.slot, jb.flags);
-    empty_arrive(0);                                                      // both buffers start empty
-    empty_arrive(1);
-#pragma unroll 1
-    for (uint64_t g = 0; g < ngroups; ++g) {
-        const uint64_t left = nblk - (g << 5);
-        const uint32_t nv = left < 32 ? (uint32_t)left : 32u;
-        const uint32_t b = (uint32_t)g & 1u;
-        full_sync(b);
-        const uint32_t *kw = kw_smem[b];
-#pragma unroll 1
-        for (uint32_t blk = 0; blk < nv; ++blk) {
-            const uint4 *kp = reinterpret_cast<const uint4 *>(kw + blk * kKwStride);
-            uint32_t v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = s[i];
-            sha_rounds4<kFma, 0>(v, kp[0], k);   sha_rounds4<kFma, 4>(v, kp[1], k);
-            sha_rounds4<kFma, 8>(v, kp[2], k);   sha_rounds4<kFma, 12>(v, kp[3], k);
-            sha_rounds4<kFma, 16>(v, kp[4], k);  sha_rounds4<kFma, 20>(v, kp[5], k);
-            sha_rounds4<kFma, 24>(v, kp[6], k);  sha_rounds4<kFma, 28>(v, kp[7], k);
-            sha_rounds4<kFma, 32>(v, kp[8], k);  sha_rounds4<kFma, 36>(v, kp[9], k);
-            sha_rounds4<kFma, 40>(v, kp[10], k); sha_rounds4<kFma, 44>(v, kp[11], k);
-            sha_rounds4<kFma, 48>(v, kp[12], k); sha_rounds4<kFma, 52>(v, kp[13], k);
-            sha_rounds4<kFma, 56>(v, kp[14], k); sha_rounds4<kFma, 60>(v, kp[15], k);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) s[i] += v[i];
-        }
-        if (g + 2 < ngroups) empty_arrive(b);                             // (nobody waits for the last two)
-    }
-    const uint64_t done = nblk << 6;
-    hash_tail<kFma>(s, jb.src + done, copy ? jb.dst + done : nullptr, (uint32_t)(jb.nbytes & 63u),
-                    (jb.flags & JOB_FINAL) != 0, jb.total_len, lane == 0, k);
-    if (lane == 0) store_state(s, states, digests, jb.slot, jb.flags);
-}
-
-// ---------------------------------------------------------------------------
-// group: S streams per warp (S = 2, 4, 8, 16), between deep (S = 1) and wide (S = 32)
-// ---------------------------------------------------------------------------
-// Same two phases as the deep kernel, with the warp's 32 lanes split as
-// lane = b * S + j: stream j, block slot b (B = 32 / S blocks per stream per
-// group).  Phase 1 is fully parallel as before (each lane expands one block);
-// phase 2 runs B dependent block-steps, every lane following stream lane % S,
-// so S round chains advance per instruction instead of one.  Lanes with the
-// same j compute identical values (no divergence); rows of the staged
-// schedule are read as S distinct 16-byte words per LDS.128 (conflict-free for
-// S <= 8, two-way for S = 16).  Streams in a warp may differ in length: a lane
-// simply stops updating its state when its stream has no block in a step.
-template <int kFma, int S>
-__global__ void __launch_bounds__(32)
-sha256_group_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *__restrict__ states,
-                    uint32_t *__restrict__ digests, FmaK k)
+template <int kFma, int S, bool kPair>
+__global__ void __launch_bounds__(kPair ? 64 : 32 * kWarpsPerCta)
+sha256_warp_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *__restrict__ states,
+                   uint32_t *__restrict__ digests, FmaK k)
 {
     constexpr uint32_t B = 32 / S;
-    __shared__ __align__(16) uint32_t kw[32 * kKwStride];
+    __shared__ __align__(16) uint32_t kw_smem[kPair ? 2 : kWarpsPerCta][32 * kKwStride];   // pairs: double-buffered
     const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t warp = threadIdx.x >> 5;                     // pairs: 0 = rounds, 1 = loads + schedules
     const uint32_t j = lane % S, b = lane / S;
-    const uint32_t job = blockIdx.x * S + j;
+    const uint32_t job = (kPair ? blockIdx.x : blockIdx.x * kWarpsPerCta + warp) * S + j;
     const bool live = job < njobs;
+    if constexpr (S == 1) {
+        if (!live) return;
+    }
     HashJob jb;
     if (live) jb = load_job(jobs, job);
     else { jb.src = nullptr; jb.dst = nullptr; jb.nbytes = 0; jb.total_len = 0; jb.slot = 0; jb.flags = JOB_INIT; jb.one = 1; jb.pad_ = 0; }
-    if constexpr (kFma == 2) k.one = jb.one;
-    uint32_t s[8];
-    load_state(s, states, jb.slot, live ? jb.flags : JOB_INIT);
-
     const uint64_t nblk = jb.nbytes >> 6;                       // this lane's stream
     uint64_t ngroups = (nblk + B - 1) / B;
+    if constexpr (S > 1) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {                          // warp-wide max: everyone loops together
-        const uint64_t other = __shfl_xor_sync(0xffffffffu, ngroups, o);
-        ngroups = other > ngroups ? other : ngroups;
+        for (int o = 16; o > 0; o >>= 1) {                      // warp-wide max: everyone loops together
+            const uint64_t other = __shfl_xor_sync(0xffffffffu, ngroups, o);
+            ngroups = other > ngroups ? other : ngroups;
+        }
     }
     const bool copy = jb.dst != nullptr;
     const uint4 *p = reinterpret_cast<const uint4 *>(jb.src) + 4ull * b;   // block b of group 0
     uint4 *q = reinterpret_cast<uint4 *>(jb.dst) + 4ull * b;
-
     uint4 x[4];
-    if (b < nblk) {
+
+    if constexpr (kPair) {
+        if (warp == 1) {
+            if (b < nblk) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
+            }
+#pragma unroll 1
+            for (uint64_t g = 0; g < ngroups; ++g) {
+                const uint32_t buf = (uint32_t)g & 1u;
+                empty_sync(buf);                                // the round warp is done with this buffer
+                stage_block<S, false>(x, p, q, copy, lane, g, ngroups, nblk,
+                                      reinterpret_cast<uint4 *>(kw_smem[buf] + lane * kKwStride));
+                __threadfence_block();                          // the stage is written before it is announced
+                full_arrive(buf);
+            }
+            return;
+        }
+    }
+
+    if constexpr (kFma == 2) k.one = jb.one;
+    uint32_t s[8];
+    load_state(s, states, jb.slot, jb.flags);
+    if constexpr (kPair) {
+        empty_arrive(0);                                        // both buffers start empty
+        empty_arrive(1);
+    } else if (b < nblk) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
     }
 #pragma unroll 1
     for (uint64_t g = 0; g < ngroups; ++g) {
         const uint64_t blk0 = g * B;
-        // phase 1: this lane's block (if its stream still has one), schedule + K into row `lane`
-        if (blk0 + b < nblk) {
-            if (copy) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) st_stream(q + i, x[i]);
-            }
-            uint32_t w[16];
-            unpack_be(w, x[0], x[1], x[2], x[3]);
-            uint4 *out = reinterpret_cast<uint4 *>(kw + lane * kKwStride);
-            expand_schedule(w, out);
-        }
-        __syncwarp();
-        p += 4 * B; q += 4 * B;
-        if (blk0 + B + b < nblk) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
-        }
-        // phase 2: B block-steps; lane follows stream j, row = step * S + j
-#pragma unroll 1
-        for (uint32_t st = 0; st < B; ++st) {
-            const bool valid = blk0 + st < nblk;
-            if (__ballot_sync(0xffffffffu, valid) == 0u) break;          // no stream has this step
-            const uint4 *kp = reinterpret_cast<const uint4 *>(kw + (st * S + j) * kKwStride);
-            uint32_t v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = s[i];
-            sha_rounds4<kFma, 0>(v, kp[0], k);   sha_rounds4<kFma, 4>(v, kp[1], k);
-            sha_rounds4<kFma, 8>(v, kp[2], k);   sha_rounds4<kFma, 12>(v, kp[3], k);
-            sha_rounds4<kFma, 16>(v, kp[4], k);  sha_rounds4<kFma, 20>(v, kp[5], k);
-            sha_rounds4<kFma, 24>(v, kp[6], k);  sha_rounds4<kFma, 28>(v, kp[7], k);
-            sha_rounds4<kFma, 32>(v, kp[8], k);  sha_rounds4<kFma, 36>(v, kp[9], k);
-            sha_rounds4<kFma, 40>(v, kp[10], k); sha_rounds4<kFma, 44>(v, kp[11], k);
-            sha_rounds4<kFma, 48>(v, kp[12], k); sha_rounds4<kFma, 52>(v, kp[13], k);
-            sha_rounds4<kFma, 56>(v, kp[14], k); sha_rounds4<kFma, 60>(v, kp[15], k);
-            if (valid) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) s[i] += v[i];
-            }
-        }
-        __syncwarp();
-    }
-    if (live) {
-        const uint64_t done = nblk << 6;
-        hash_tail<kFma>(s, jb.src + done, copy ? jb.dst + done : nullptr, (uint32_t)(jb.nbytes & 63u),
-                        (jb.flags & JOB_FINAL) != 0, jb.total_len, b == 0, k);
-        if (b == 0) store_state(s, states, digests, jb.slot, jb.flags);
-    }
-}
-
-// group2: the group kernel with the deep2 split - warp 1 loads, copies out and expands the next group's 32 blocks
-// (lane = block_slot * S + stream, as in the group kernel) while warp 0 runs the current group's 32 / S block-steps for
-// its S streams.  In the group kernel phase 1 is not a 4 % matter as in the deep kernel: per group of 32 blocks it
-// costs ~1500 cycles against (32 / S) x ~1600 for the rounds - 19 % of the time at S = 8, 32 % at S = 16.
-template <int kFma, int S>
-__global__ void __launch_bounds__(64)
-sha256_group2_kernel(const HashJob *__restrict__ jobs, uint32_t njobs, uint32_t *__restrict__ states,
-                     uint32_t *__restrict__ digests, FmaK k)
-{
-    constexpr uint32_t B = 32 / S;
-    __shared__ __align__(16) uint32_t kw_smem[2][32 * kKwStride];
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t role = threadIdx.x >> 5;                     // 0: rounds, 1: loads + schedules
-    const uint32_t j = lane % S, b = lane / S;
-    const uint32_t job = blockIdx.x * S + j;
-    const bool live = job < njobs;
-    HashJob jb;
-    if (live) jb = load_job(jobs, job);
-    else { jb.src = nullptr; jb.dst = nullptr; jb.nbytes = 0; jb.total_len = 0; jb.slot = 0; jb.flags = JOB_INIT; jb.one = 1; jb.pad_ = 0; }
-    const uint64_t nblk = jb.nbytes >> 6;                       // this lane's stream
-    uint64_t ngroups = (nblk + B - 1) / B;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {                          // warp-wide max (both warps arrive at the same number)
-        const uint64_t other = __shfl_xor_sync(0xffffffffu, ngroups, o);
-        ngroups = other > ngroups ? other : ngroups;
-    }
-    const bool copy = jb.dst != nullptr;
-
-    if (role == 1) {
-        const uint4 *p = reinterpret_cast<const uint4 *>(jb.src) + 4ull * b;
-        uint4 *q = reinterpret_cast<uint4 *>(jb.dst) + 4ull * b;
-        uint4 x[4];
-        if (b < nblk) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
-        }
-#pragma unroll 1
-        for (uint64_t g = 0; g < ngroups; ++g) {
-            const uint64_t blk0 = g * B;
-            const uint32_t buf = (uint32_t)g & 1u;
-            empty_sync(buf);
-            if (blk0 + b < nblk) {
-                if (copy) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) st_stream(q + i, x[i]);
-                }
-                uint32_t w[16];
-                unpack_be(w, x[0], x[1], x[2], x[3]);
-                expand_schedule(w, reinterpret_cast<uint4 *>(kw_smem[buf] + lane * kKwStride));
-            }
-            p += 4 * B; q += 4 * B;
-            if (blk0 + B + b < nblk) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) x[i] = ld_stream(p + i);
-            }
-            __threadfence_block();
-            full_arrive(buf);
-        }
-        return;
-    }
-
-    uint32_t s[8];
-    load_state(s, states, jb.slot, live ? jb.flags : JOB_INIT);
-    empty_arrive(0);
-    empty_arrive(1);
-#pragma unroll 1
-    for (uint64_t g = 0; g < ngroups; ++g) {
-        const uint64_t blk0 = g * B;
         const uint32_t buf = (uint32_t)g & 1u;
-        full_sync(buf);
-        const uint32_t *kw = kw_smem[buf];
+        if constexpr (kPair) {
+            full_sync(buf);
+        } else {
+            // the next group's block is loaded while the serial rounds run
+            stage_block<S, true>(x, p, q, copy, lane, g, ngroups, nblk,
+                                 reinterpret_cast<uint4 *>(kw_smem[warp] + lane * kKwStride));
+        }
+        const uint32_t *kw = kw_smem[kPair ? buf : warp];
+        if constexpr (S == 1) {
+            const uint64_t left = nblk - blk0;
+            const uint32_t nv = left < 32 ? (uint32_t)left : 32u;
 #pragma unroll 1
-        for (uint32_t st = 0; st < B; ++st) {
-            const bool valid = blk0 + st < nblk;
-            if (__ballot_sync(0xffffffffu, valid) == 0u) break;          // no stream has this step
-            const uint4 *kp = reinterpret_cast<const uint4 *>(kw + (st * S + j) * kKwStride);
-            uint32_t v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = s[i];
-            sha_rounds4<kFma, 0>(v, kp[0], k);   sha_rounds4<kFma, 4>(v, kp[1], k);
-            sha_rounds4<kFma, 8>(v, kp[2], k);   sha_rounds4<kFma, 12>(v, kp[3], k);
-            sha_rounds4<kFma, 16>(v, kp[4], k);  sha_rounds4<kFma, 20>(v, kp[5], k);
-            sha_rounds4<kFma, 24>(v, kp[6], k);  sha_rounds4<kFma, 28>(v, kp[7], k);
-            sha_rounds4<kFma, 32>(v, kp[8], k);  sha_rounds4<kFma, 36>(v, kp[9], k);
-            sha_rounds4<kFma, 40>(v, kp[10], k); sha_rounds4<kFma, 44>(v, kp[11], k);
-            sha_rounds4<kFma, 48>(v, kp[12], k); sha_rounds4<kFma, 52>(v, kp[13], k);
-            sha_rounds4<kFma, 56>(v, kp[14], k); sha_rounds4<kFma, 60>(v, kp[15], k);
-            if (valid) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) s[i] += v[i];
+            for (uint32_t st = 0; st < nv; ++st) block_step<kFma>(s, reinterpret_cast<const uint4 *>(kw + st * kKwStride), true, k);
+        } else {
+#pragma unroll 1
+            for (uint32_t st = 0; st < B; ++st) {              // row = step * S + j
+                const bool valid = blk0 + st < nblk;
+                if (__ballot_sync(0xffffffffu, valid) == 0u) break;          // no stream has this step
+                block_step<kFma>(s, reinterpret_cast<const uint4 *>(kw + (st * S + j) * kKwStride), valid, k);
             }
         }
-        if (g + 2 < ngroups) empty_arrive(buf);
+        if constexpr (kPair) {
+            if (g + 2 < ngroups) empty_arrive(buf);             // (nobody waits for the last two)
+        } else {
+            __syncwarp();
+        }
     }
     if (live) {
         const uint64_t done = nblk << 6;
@@ -836,97 +627,41 @@ static void launch_wide_t(const HashJob *jobs, uint32_t njobs, uint32_t *states,
     sha256_wide_kernel<kFma, kStyle><<<grid, kWideThreads, 0, stream>>>(jobs, njobs, states, digests, kFmaK);
 }
 
-// variant = fma + 4 * style   (fma 0..3, style 0..4)
-cudaError_t launch_sha256_wide(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests,
-                               cudaStream_t stream, int variant)
+template <int kFma, int S, bool kPair>
+static void launch_warp_t(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests, cudaStream_t stream)
+{
+    constexpr uint32_t per_cta = kPair ? S : S * kWarpsPerCta;
+    sha256_warp_kernel<kFma, S, kPair><<<(njobs + per_cta - 1) / per_cta, kPair ? 64 : 32 * kWarpsPerCta, 0, stream>>>(
+        jobs, njobs, states, digests, kFmaK);
+}
+
+// One case label per built kernel; -1 for fields no kernel has.
+static constexpr int shape_key(int spw, bool pairs, int form)
+{
+    return spw >= 1 && spw <= 32 && form >= 0 && form < 32 ? (spw * 2 + (pairs ? 1 : 0)) * 32 + form : -1;
+}
+
+cudaError_t launch_sha256(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests,
+                          cudaStream_t stream, const KernelShape &shape)
 {
     if (njobs == 0) return cudaSuccess;
     clear_stale_error();
-    switch (variant) {
-#define DM_W(f, st) case (f) + 4 * (st): launch_wide_t<f, st>(jobs, njobs, states, digests, stream); break;
+    switch (shape_key(shape.spw, shape.pairs, shape.form)) {
+#define DM_W(f, st) case shape_key(32, false, (f) + 4 * (st)): launch_wide_t<f, st>(jobs, njobs, states, digests, stream); break;
     DM_W(0, 0) DM_W(1, 0) DM_W(2, 0) DM_W(0, 1) DM_W(1, 1) DM_W(2, 1)
     DM_W(0, 2) DM_W(1, 2) DM_W(2, 2) DM_W(0, 3) DM_W(1, 3) DM_W(2, 3)
     DM_W(0, 4) DM_W(1, 4) DM_W(2, 4)
     DM_W(1, 5)
 #undef DM_W
-    default: launch_wide_t<kDefaultWideVariant % 4, kDefaultWideVariant / 4>(jobs, njobs, states, digests, stream); break;
-    }
-    return cudaGetLastError();
-}
-
-cudaError_t launch_sha256_deep(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests,
-                               cudaStream_t stream, int variant)
-{
-    if (njobs == 0) return cudaSuccess;
-    const uint32_t grid = (njobs + kDeepWarps - 1) / kDeepWarps;
-    clear_stale_error();
-    if (variant == 9) variant = 8;                     // (9 = two-warp group kernels too; the deep kernel's own rule is 8's)
-    if (variant == 8 && njobs > kMaxWarpPairs) variant = 7;
-    if (variant == 10) variant = 8;                    // 10 = two warps per stream whatever the count (A/B of the 264 rule)      // two warps per stream only while each still gets a sub-partition of its own
-    switch (variant) {
-    case 1: case 3: sha256_deep_kernel<1><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 2: sha256_deep_kernel<2><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 4: sha256_deep_kernel<4><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 5: sha256_deep_kernel<5><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 6: sha256_deep_kernel<6><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 7: sha256_deep_kernel<7><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    // 8: form 7 with a schedule warp running ahead of the round warp (two warps per stream; callers keep it to
-    //    launches of at most 264 jobs, so that every warp has a sub-partition of its own)
-    case 8: sha256_deep2_kernel<7><<<njobs, 64, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    default: sha256_deep_kernel<0><<<grid, 32 * kDeepWarps, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    }
-    return cudaGetLastError();
-}
-
-// streams_per_warp in {2, 4, 8, 16}; variant 4 = the short-chain round (see sha256_round.cuh), else ptxas' own
-template <int kFma>
-static cudaError_t launch_group2_t(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests,
-                                   cudaStream_t stream, int streams_per_warp)
-{
-    const uint32_t spw = (uint32_t)streams_per_warp;
-    const uint32_t grid = (njobs + spw - 1) / spw;
-    switch (streams_per_warp) {
-    case 2: sha256_group2_kernel<kFma, 2><<<grid, 64, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 4: sha256_group2_kernel<kFma, 4><<<grid, 64, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 8: sha256_group2_kernel<kFma, 8><<<grid, 64, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 16: sha256_group2_kernel<kFma, 16><<<grid, 64, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
+#define DM_S(f, s, pr) case shape_key(s, pr, f): launch_warp_t<f, s, pr>(jobs, njobs, states, digests, stream); break;
+#define DM_S_ALL(f, pr) DM_S(f, 1, pr) DM_S(f, 2, pr) DM_S(f, 4, pr) DM_S(f, 8, pr) DM_S(f, 16, pr)
+    DM_S_ALL(0, false) DM_S(1, 1, false) DM_S(2, 1, false) DM_S_ALL(4, false) DM_S_ALL(5, false) DM_S_ALL(6, false)
+    DM_S_ALL(7, false) DM_S_ALL(7, true)
+#undef DM_S_ALL
+#undef DM_S
     default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();
-}
-
-template <int kFma>
-static cudaError_t launch_group_t(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests,
-                                  cudaStream_t stream, int streams_per_warp)
-{
-    const uint32_t spw = (uint32_t)streams_per_warp;
-    const uint32_t grid = (njobs + spw - 1) / spw;
-    switch (streams_per_warp) {
-    case 2: sha256_group_kernel<kFma, 2><<<grid, 32, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 4: sha256_group_kernel<kFma, 4><<<grid, 32, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 8: sha256_group_kernel<kFma, 8><<<grid, 32, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    case 16: sha256_group_kernel<kFma, 16><<<grid, 32, 0, stream>>>(jobs, njobs, states, digests, kFmaK); break;
-    default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
-}
-
-cudaError_t launch_sha256_group(const HashJob *jobs, uint32_t njobs, uint32_t *states, uint32_t *digests,
-                                cudaStream_t stream, int streams_per_warp, int variant)
-{
-    if (njobs == 0) return cudaSuccess;
-    clear_stale_error();
-    switch (variant) {
-    case 4: return launch_group_t<4>(jobs, njobs, states, digests, stream, streams_per_warp);
-    case 5: return launch_group_t<5>(jobs, njobs, states, digests, stream, streams_per_warp);
-    case 6: return launch_group_t<6>(jobs, njobs, states, digests, stream, streams_per_warp);
-    case 7: case 8: case 10: return launch_group_t<7>(jobs, njobs, states, digests, stream, streams_per_warp);
-    case 9:                                             // two warps per group of S streams, while every pair can have two sub-partitions
-        if ((njobs + (uint32_t)streams_per_warp - 1) / (uint32_t)streams_per_warp <= kMaxWarpPairs)
-            return launch_group2_t<7>(jobs, njobs, states, digests, stream, streams_per_warp);
-        return launch_group_t<7>(jobs, njobs, states, digests, stream, streams_per_warp);
-    default: return launch_group_t<0>(jobs, njobs, states, digests, stream, streams_per_warp);
-    }
 }
 
 cudaError_t launch_synth_fill(uint64_t seed, uint64_t blob, uint64_t byte_off, void *dst, size_t len,

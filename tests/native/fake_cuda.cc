@@ -1,5 +1,5 @@
-// TEST INFRASTRUCTURE ONLY — see fake_cuda/cuda_runtime.h.  Asynchronous fake runtime (one worker thread per stream) + the three
-// SHA-256 "kernel" launchers executed on the CPU by the oracle (oracle/sha256_oracle.c), honouring
+// TEST INFRASTRUCTURE ONLY — see fake_cuda/cuda_runtime.h.  Asynchronous fake runtime (one worker thread per stream) + the
+// SHA-256 "kernel" launcher executed on the CPU by the oracle (oracle/sha256_oracle.c), honouring
 // exactly the HashJob contract the real kernels implement (INIT / FINAL flags, state table, fused copy).
 #include "fake_cuda/cuda_runtime.h"
 #include "../../demodel_b200/csrc/sha256_kernels.cuh"
@@ -336,9 +336,7 @@ static cudaError_t run_all(const HashJob *jobs, uint32_t n, uint32_t *states, ui
     on_stream(st, [jobs, n, states, digests] { for (uint32_t i = 0; i < n; ++i) run_job(jobs[i], states, digests); });
     return cudaGetLastError();                   // as the real launch wrappers end (sha256_kernels.cu)
 }
-cudaError_t launch_sha256_wide(const HashJob *j, uint32_t n, uint32_t *s, uint32_t *d, cudaStream_t st, int) { return run_all(j, n, s, d, st); }
-cudaError_t launch_sha256_deep(const HashJob *j, uint32_t n, uint32_t *s, uint32_t *d, cudaStream_t st, int) { return run_all(j, n, s, d, st); }
-cudaError_t launch_sha256_group(const HashJob *j, uint32_t n, uint32_t *s, uint32_t *d, cudaStream_t st, int, int) { return run_all(j, n, s, d, st); }
+cudaError_t launch_sha256(const HashJob *j, uint32_t n, uint32_t *s, uint32_t *d, cudaStream_t st, const KernelShape &) { return run_all(j, n, s, d, st); }
 
 cudaError_t launch_synth_fill(uint64_t seed, uint64_t blob, uint64_t off, void *dst, size_t len, cudaStream_t st)
 {

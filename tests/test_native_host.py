@@ -139,6 +139,18 @@ def test_every_round_form_is_sha256_on_the_host(tmp_path):
     assert out.returncode == 0 and "ROUND FORMS OK" in out.stdout, out.stdout + out.stderr
 
 
+def test_kernel_shape_choice_on_the_host(tmp_path):
+    """kernel_shape() compiled by g++ against the fake CUDA headers: the variant -> round form mapping and the
+    warp-pair rule (8 pairs S = 1, 9 any S <= 16, both only while the groups fit in 264 pairs; 10 pairs S = 1
+    whatever the count; a pair count of 0 never pairs), which otherwise shows only through digests on a GPU."""
+    exe = tmp_path / "kernel_shape"
+    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "tests", "native", "fake_cuda"),
+                    "-I", os.path.join(ROOT, "demodel_b200", "csrc"), "-o", str(exe),
+                    os.path.join(ROOT, "tests", "native", "test_kernel_shape.cc")], check=True)
+    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=60)
+    assert out.returncode == 0 and "KERNEL SHAPE OK" in out.stdout, out.stdout + out.stderr
+
+
 def test_python_mirror_gpu_test_logic_and_bench_flow_over_the_fake_runtime(tmp_path):
     """The host-buffer tests of test_gpu_parity.py / test_manifest.py, run here against the engine built over the
     fake CUDA runtime (its 'kernels' are the CPU oracle): exercises the ctypes mirror and the tests' own logic on
@@ -179,7 +191,7 @@ def test_python_mirror_gpu_test_logic_and_bench_flow_over_the_fake_runtime(tmp_p
 
 
 def test_sass_timing_model_ranks_the_short_chain_round_ahead(tmp_path):
-    """tools/sass_sched.py on the built sm_90a kernels: ptxas' own ordering of the deep kernel's serial phase must come
+    """tools/sass_sched.py on the built sm_90a kernels: ptxas' own ordering of the one-warp-per-stream serial phase must come
     out at the model's 35 cycles per round, and the short-chain candidate must be predicted faster.  On an H100 SXM
     (1.98 GHz) the two measure 37.8 and 26.5 cycles per round (deep variants 0 and 7, 256 x 1 MiB): the model leaves
     out what the hardware adds (dispatch, LDS arrival), so it ranks round forms rather than predicting their time."""
@@ -193,8 +205,8 @@ def test_sass_timing_model_ranks_the_short_chain_round_ahead(tmp_path):
     with open(sass, "w") as f:
         subprocess.run(["cuobjdump", "-sass", obj], stdout=f, check=True, timeout=300)
     cyc = {}
-    for v in (0, 4):
-        out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "sass_sched.py"), str(sass), f"deep_kernelILi{v}E"],
+    for v in (0, 4):                              # one warp per stream: sha256_warp_kernel<v, 1, false>
+        out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "sass_sched.py"), str(sass), f"warp_kernelILi{v}ELi1ELb0EE"],
                              capture_output=True, text=True, timeout=300)
         assert out.returncode == 0, out.stderr
         cyc[v] = float(re.search(r"= ([0-9.]+) cycles per round", out.stdout).group(1))

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Static issue-timing estimate for a straight-line SASS loop run by ONE warp.
 
-For the single-warp serial phase of the deep kernel (one warp per stream, alone on
+For the single-warp serial phase of sha256_warp_kernel (one warp per stream, alone on
 its sub-partition) nothing hides latency, so the cycles per round can be estimated
 from the SASS alone.  Model (pipe rates and latencies as tools/ubench/pipemix.cu and
 chainlat.cu measure them):
@@ -14,13 +14,13 @@ chainlat.cu measure them):
 
 Usage:
   cuobjdump -sass build/sha256_kernels.o > all.sass
-  tools/sass_sched.py all.sass 'deep_kernelILi0E' [--iters 3]
+  tools/sass_sched.py all.sass 'warp_kernelILi0ELi1ELb0EE' [--iters 3]   # <form 0, S = 1, one warp>
 
 Picks the loop between the first and last LDS of the named function (the phase-2
 block loop), replays it `iters` times and prints cycles per iteration in steady
 state, the pipe-issue lower bounds and the critical-path bound.  It is a ranking
 tool for candidate round orderings when no GPU is at hand.  On an H100 SXM the
-model reads 35.0 cycles per round for deep<0> and 24.3 for deep<7>; measured at
+model reads 35.0 cycles per round for form 0 and 24.3 for form 7 at S = 1; measured at
 1.98 GHz (256 x 1 MiB per launch) they take 37.8 and 26.5.
 """
 import argparse

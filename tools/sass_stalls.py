@@ -1,14 +1,14 @@
 #!/usr/bin/env python3
 """Cycles per iteration that ptxas itself scheduled: sum of the stall counts in the SASS control words.
 
-For a single in-order warp running fixed-latency integer code (the deep / group kernels' serial phase) the
+For a single in-order warp running fixed-latency integer code (sha256_warp_kernel's serial phase) the
 issue time of the loop is, to first order, the sum over its instructions of the `stall` field ptxas encoded
 (bits 105..108 of each 128-bit instruction: cycles to wait before issuing the next one) - ncu shows exactly
 that for the shipped kernel: `selected` 1.00 + `wait` 1.02 per issue and nothing else
 (ncu metrics of the deep kernel).  Comparing this number with the measured launch time says whether
 a form is limited by ptxas' own schedule or by something the hardware adds on top.
 
-  cuobjdump -sass build/sha256_kernels.o > all.sass; tools/sass_stalls.py all.sass 'deep_kernelILi7E'
+  cuobjdump -sass build/sha256_kernels.o > all.sass; tools/sass_stalls.py all.sass 'warp_kernelILi7ELi1ELb0EE'
 """
 import collections
 import re
