@@ -18,6 +18,7 @@ DM_OK, DM_EINVAL, DM_ENOMEM, DM_ENOENT, DM_ECUDA, DM_ESTATE, DM_EIO, DM_ENODEV, 
 DM_F_NO_HBM_CAS = 0x1
 DM_F_DISK_SYNC = 0x2
 DM_F_NUMA_LOCAL = 0x4
+DM_F_DISK_DIRECT = 0x8
 DM_ING_HASH_ONLY = 0x1
 DM_ING_REPLACE = 0x2
 DM_ING_FORCE_WIDE = 0x4

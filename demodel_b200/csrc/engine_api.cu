@@ -3,6 +3,7 @@
 
 #include <dirent.h>
 #include <sched.h>
+#include <signal.h>
 
 namespace {
 
@@ -43,6 +44,22 @@ bool numa_cpus_of_device(int device, cpu_set_t *set, int *node_out)
     }
     *node_out = node;
     return n_set > 0;
+}
+
+// Files of disk-backed streams are named <pid>-<device>-<id>.part: remove those of processes that are gone, and
+// leave every live process's alone (other engines may share the directory).
+void sweep_incoming(const std::string &dir)
+{
+    DIR *d = opendir(dir.c_str());
+    if (!d) return;
+    while (struct dirent *de = readdir(d)) {
+        char *end = nullptr;
+        const long pid = strtol(de->d_name, &end, 10);
+        if (end == de->d_name || *end != '-' || pid <= 0) continue;
+        if (kill((pid_t)pid, 0) == 0 || errno == EPERM) continue;        // alive (EPERM: alive, another user's)
+        unlink((dir + "/" + de->d_name).c_str());
+    }
+    closedir(d);
 }
 
 }  // namespace
@@ -137,6 +154,12 @@ void dm_engine_destroy(dm_engine *e)
     }
     e->spill_cv.notify_all();
     for (auto &t : e->spillers) if (t.joinable()) t.join();
+    { std::lock_guard<std::mutex> g(e->disk_mu); e->disk_stop = true; }     // after the completers: they queue publications
+    e->disk_cv.notify_all();
+    for (auto &t : e->disk_threads) if (t.joinable()) t.join();
+    for (auto &m : e->streams)                    // disk-backed streams nobody finished: their files go with the engine
+        for (auto &kv : m)
+            if (kv.second->fd >= 0) { close(kv.second->fd); unlink(kv.second->path.c_str()); }
     cudaDeviceSynchronize();
     for (auto &m : e->readers) for (auto &kv : m) if (kv.second->fd >= 0) close(kv.second->fd);
     for (Cycle &c : e->cycles) {
@@ -192,6 +215,7 @@ static int engine_create(const dm_config *cfg, dm_engine **out)
     }
     if (cfg->device < 0 || cfg->device >= ndev) return fail(DM_ENODEV, "device ordinal out of range");
     if (cfg->slab_bytes && (cfg->slab_bytes % 256)) return fail(DM_EINVAL, "slab_bytes must be a multiple of 256");
+    if ((cfg->flags & DM_F_DISK_DIRECT) && !(cfg->cas_dir && cfg->cas_dir[0])) return fail(DM_EINVAL, "DM_F_DISK_DIRECT needs a cas_dir");
 
     dm_engine *e = new dm_engine();
     e->cfg = *cfg;
@@ -321,8 +345,14 @@ static int engine_create(const dm_config *cfg, dm_engine **out)
             }
             closedir(dir);
         }
+        if (e->cfg.flags & DM_F_DISK_DIRECT) {
+            mkdirs(e->cas_dir + "/incoming/x");
+            sweep_incoming(e->cas_dir + "/incoming");
+        }
     }
     e->pump = std::thread(pump_main, e);
+    if (e->cfg.flags & DM_F_DISK_DIRECT)
+        for (int i = 0; i < kDiskThreads; ++i) e->disk_threads.emplace_back(disk_main, e);
     for (int i = 0; i < kCompleters; ++i) e->completers.emplace_back(completer_main, e);
     if (!e->cas_dir.empty())
         for (int i = 0; i < kSpillThreads; ++i) e->spillers.emplace_back(spill_main, e);
@@ -380,6 +410,16 @@ static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t siz
             return rc;
         }
         sp->verify_only = true;
+    }
+    if (sp->verify_only && (e->cfg.flags & DM_F_DISK_DIRECT)) {      // kept after all: in a file of the disk tier
+        sp->disk = true;
+        sp->path = incoming_path(e, sp->id);
+        sp->fd = open(sp->path.c_str(), O_CREAT | O_TRUNC | O_RDWR | O_CLOEXEC, 0644);
+        if (sp->fd < 0) {
+            std::lock_guard<std::mutex> g2(e->slot_mu);
+            e->free_slots.push_back(sp->slot);
+            return fail(DM_EIO, "could not create the stream's file under <cas_dir>/incoming");
+        }
     }
     if (size_hint && !sp->verify_only) {
         cudaSetDevice(e->device);
@@ -483,7 +523,7 @@ static int stream_write_at_impl(dm_engine *e, uint64_t id, uint64_t offset, cons
         g.unlock();
         return stream_write_impl(e, id, buf, len);          // plain sequential continuation
     }
-    if (s->verify_only) return fail(DM_ESTATE, "out-of-order ranges need the HBM store (engine is verify-only)");
+    if (s->verify_only && !s->disk) return fail(DM_ESTATE, "out-of-order ranges need the HBM store (engine is verify-only)");
     const uint8_t *p = static_cast<const uint8_t *>(buf);
     const uint32_t slab_bytes = e->cfg.slab_bytes;
     while (len) {
@@ -530,6 +570,24 @@ static int stream_write_at_impl(dm_engine *e, uint64_t id, uint64_t offset, cons
     return DM_OK;
 }
 
+// The SHA-256 chaining value in state slot `slot` after `hashed` bytes (the IV when nothing is hashed).  No job of
+// the stream may be running.  Used by dm_stream_checkpoint and by the suspend of a disk-backed stream.
+static int read_chain_state(dm_engine *e, uint32_t slot, uint64_t hashed, uint32_t h[8])
+{
+    if (hashed == 0) {
+        static const uint32_t iv[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au,
+                                       0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+        memcpy(h, iv, sizeof iv);
+        return DM_OK;
+    }
+    cudaSetDevice(e->device);
+    std::lock_guard<std::mutex> gc(e->ckpt_mu);
+    CU_TRY(cudaMemcpyAsync(e->ckpt_pinned, e->d_states + 8ull * slot, 32, cudaMemcpyDeviceToHost, e->ckpt_stream));
+    CU_TRY(cudaStreamSynchronize(e->ckpt_stream));
+    memcpy(h, e->ckpt_pinned, 32);
+    return DM_OK;
+}
+
 static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out)
 {
     if (!e || !out) return fail(DM_EINVAL, "null argument");
@@ -545,7 +603,7 @@ static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out)
         if (rc != DM_OK) return rc;
         if (s->st != St::Open) return fail(DM_ESTATE, "stream closed during checkpoint");
     }
-    if (!s->verify_only || (s->cur_fill & 63) == 0) {
+    if (!s->verify_only || s->disk || (s->cur_fill & 63) == 0) {
         // push out what is staged so the checkpoint covers every whole block received in order
         // (a verify-only stream hashes slab by slab, so only a block-aligned partial slab may go early)
         int rc = submit_slab(e, sp);
@@ -553,7 +611,10 @@ static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out)
     }
     // everything DMA'd so far in whole blocks must be hashed and no job may be running
     s->ckpt_waiter = true;
-    s->cv.wait(g, [&] { return s->st != St::Open || (s->jobs_inflight == 0 && ((s->dma_issued - s->hash_issued) & ~63ull) == 0); });
+    s->cv.wait(g, [&] {
+        return s->st != St::Open || (s->disk && s->lost != DM_OK) ||      // (a failed file write leaves a hole the hash never passes)
+               (s->jobs_inflight == 0 && ((s->dma_issued - s->hash_issued) & ~63ull) == 0);
+    });
     s->ckpt_waiter = false;
     if (s->st != St::Open) return fail(DM_ESTATE, "stream closed during checkpoint");
     if (s->cuda_failed) return fail(DM_ECUDA, "a CUDA copy or launch failed on this stream: its state is not trusted");
@@ -561,18 +622,7 @@ static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out)
     memset(out, 0, sizeof *out);
     out->abi = DM_ABI_VERSION;
     out->bytes = s->hash_issued;
-    if (s->hash_issued == 0) {
-        static const uint32_t iv[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au,
-                                       0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
-        memcpy(out->h, iv, sizeof iv);
-        return DM_OK;
-    }
-    cudaSetDevice(e->device);
-    std::lock_guard<std::mutex> gc(e->ckpt_mu);
-    CU_TRY(cudaMemcpyAsync(e->ckpt_pinned, e->d_states + 8ull * s->slot, 32, cudaMemcpyDeviceToHost, e->ckpt_stream));
-    CU_TRY(cudaStreamSynchronize(e->ckpt_stream));
-    memcpy(out->h, e->ckpt_pinned, 32);
-    return DM_OK;
+    return read_chain_state(e, s->slot, s->hash_issued, out->h);
 }
 
 static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id);
@@ -593,7 +643,7 @@ static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8
     if (!sp) return fail(DM_ESTATE, "stream closed while resuming");
     Stream *s = sp.get();
     std::unique_lock<std::mutex> g(s->mu);
-    s->resume_base = s->dma_issued = s->hash_issued = s->landed = ck->bytes;
+    s->resume_base = s->dma_issued = s->hash_issued = s->landed = s->staged_to = ck->bytes;
     if (ck->bytes == 0 && s->has_expect && !s->verify_only) {
         std::lock_guard<std::mutex> g2(e->mu);
         auto &slot = e->inflight[s->expect];
@@ -611,6 +661,7 @@ static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8
         if (err != cudaSuccess) {
             // nothing of this stream is in flight yet: give back its extent, state slot and id
             s->st = St::Aborted;
+            if (s->disk) { close(s->fd); s->fd = -1; unlink(s->path.c_str()); }
             g.unlock();
             free_extents(e, s->extents);
             drop_stream(e, sp, true);
@@ -636,12 +687,98 @@ struct SavedCkpt {
     uint8_t expect[32];
 };
 const char kCkptMagic[8] = {'D', 'M', 'C', 'K', 'P', 'T', 0, 2};
+// A disk-backed stream's record: the hash stopped at ck.bytes, the .part holds the first `saved` bytes (saved >= ck.bytes)
+struct SavedDiskCkpt {
+    SavedCkpt ck;           // magic "DMCKPT\0\3"
+    uint64_t saved;         // multiple of 64
+};
+const char kDiskCkptMagic[8] = {'D', 'M', 'C', 'K', 'P', 'T', 0, 3};
 std::string partial_base(const dm_engine *e, const uint8_t d[32]) { return e->cas_dir + "/partial/" + hex_of(d, 32); }
 }  // namespace
 
 static int stream_abort_impl(dm_engine *e, uint64_t id);
 static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out);
 static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id);
+
+// dm_stream_suspend of a disk-backed stream: no wait for the hash, no copy.  The state at the hashed position H
+// is saved with H and C (the contiguous written prefix, rounded down to 64); the file, cut to C, is renamed.
+static int suspend_disk(dm_engine *e, const std::shared_ptr<Stream> &sp, uint64_t *resume_from)
+{
+    Stream *s = sp.get();
+    uint64_t hashed, saved, hint;
+    int fd;
+    std::string path;
+    auto unsuspend = [&](std::unique_lock<std::mutex> &g) { s->suspending = false; disk_feed(e, sp); mark_dirty(e, sp, nullptr); g.unlock(); };
+    {
+        std::unique_lock<std::mutex> g(s->mu);
+        if (s->st != St::Open || s->window_out) return fail(DM_ESTATE, "stream not open");
+        int rc = submit_slab(e, sp);                      // what sits in the ring goes to the file first
+        while (rc == DM_OK && !s->parts.empty()) rc = submit_part(e, sp, s->parts.size() - 1);
+        if (rc != DM_OK) return rc;
+        s->suspending = true;
+        s->ckpt_waiter = true;
+        s->cv.wait(g, [&] { return s->st != St::Open || (s->jobs_inflight == 0 && s->disk_writes == 0 && s->disk_reads == 0); });
+        s->ckpt_waiter = false;
+        if (s->st != St::Open) return fail(DM_ESTATE, "stream closed during suspend");
+        if (s->cuda_failed) { unsuspend(g); return fail(DM_ECUDA, "a CUDA copy or launch failed on this stream: its state is not trusted"); }
+        if (s->lost != DM_OK) { unsuspend(g); return fail(s->lost, kLostText); }
+        if (!s->staged.empty()) {                         // read back but not hashed: the resumed stream reads them again
+            cudaSetDevice(e->device);
+            cudaStreamSynchronize(e->copy_stream[s->id % kCopyStreams]);
+            for (auto &ps : s->staged) slab_return(e, ps.first);
+            s->staged.clear();
+        }
+        s->staged_to = s->hash_issued;
+        hashed = s->hash_issued;
+        saved = 0;
+        if (!s->written.empty() && s->written.begin()->first == 0) saved = s->written.begin()->second & ~63ull;
+        hint = s->size_hint;
+        fd = s->fd;
+        path = s->path;
+    }
+    dm_checkpoint ck;
+    memset(&ck, 0, sizeof ck);
+    ck.bytes = hashed;
+    if (int rc = read_chain_state(e, s->slot, hashed, ck.h); rc != DM_OK) {
+        std::unique_lock<std::mutex> g(s->mu);
+        unsuspend(g);
+        return rc;
+    }
+    const std::string base = partial_base(e, s->expect.b);
+    SavedDiskCkpt rec;
+    memset(&rec, 0, sizeof rec);
+    memcpy(rec.ck.magic, kDiskCkptMagic, 8);
+    rec.ck.abi = DM_ABI_VERSION; rec.ck.bytes = hashed; rec.ck.size_hint = hint; rec.saved = saved;
+    memcpy(rec.ck.h, ck.h, sizeof rec.ck.h);
+    memcpy(rec.ck.expect, s->expect.b, 32);
+    struct stat st;
+    const bool fresh = stat((base + ".ckpt").c_str(), &st) != 0;
+    unlink((base + ".ckpt").c_str());                    // an older record must not pair with the new bytes
+    bool ok = ftruncate(fd, (off_t)saved) == 0 && rename(path.c_str(), (base + ".part").c_str()) == 0;
+    const bool moved = ok;
+    FILE *f = ok ? fopen((base + ".ckpt.tmp").c_str(), "wb") : nullptr;
+    ok = f && fwrite(&rec, sizeof rec, 1, f) == 1 && fflush(f) == 0;
+    if (f) fclose(f);
+    ok = ok && rename((base + ".ckpt.tmp").c_str(), (base + ".ckpt").c_str()) == 0;
+    if (!ok) {
+        unlink((base + ".ckpt.tmp").c_str());
+        if (moved) rename((base + ".part").c_str(), path.c_str());     // the stream keeps its file
+        if (!fresh && e->n_suspended) e->n_suspended--;               // the older record went with the attempt
+        std::unique_lock<std::mutex> g(s->mu);
+        unsuspend(g);
+        return fail(DM_EIO, "could not save the checkpoint under <cas_dir>/partial (the stream is still open)");
+    }
+    {
+        std::lock_guard<std::mutex> g(s->mu);            // the file is the saved download now, not the stream's
+        close(s->fd);
+        s->fd = -1;
+        s->path.clear();
+    }
+    if (fresh) e->n_suspended++;
+    stream_abort_impl(e, s->id);                         // releases the id, the state slot and the staged slabs
+    if (resume_from) *resume_from = saved;
+    return DM_OK;
+}
 
 static int stream_suspend_impl(dm_engine *e, uint64_t id, uint64_t *resume_from)
 {
@@ -651,15 +788,18 @@ static int stream_suspend_impl(dm_engine *e, uint64_t id, uint64_t *resume_from)
     auto sp = find_stream(e, id);
     if (!sp) return fail(DM_EINVAL, "unknown stream id");
     Stream *s = sp.get();
+    bool disk;
     {
         std::lock_guard<std::mutex> g(s->mu);
         if (!s->has_expect) return fail(DM_ESTATE, "only a stream opened with an expected digest can be suspended (the digest names the saved files)");
-        if (s->verify_only) return fail(DM_ESTATE, "a verify-only stream retains no bytes to save");
+        if (s->verify_only && !s->disk) return fail(DM_ESTATE, "a verify-only stream retains no bytes to save");
         const bool whole = s->resume_base == 0 ||
                            (s->prefix_cover.size() == 1 && s->prefix_cover.begin()->first == 0 &&
                             s->prefix_cover.begin()->second >= s->resume_base);
         if (!whole) return fail(DM_ESTATE, "the stream was resumed without its prefix: there is nothing whole to save");
+        disk = s->disk;
     }
+    if (disk) return suspend_disk(e, sp, resume_from);
     dm_checkpoint ck;
     int rc = stream_checkpoint_impl(e, id, &ck);        // every whole block received in order is hashed now
     if (rc != DM_OK) return rc;
@@ -717,12 +857,19 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
     if (e->cas_dir.empty()) return DM_ENOENT;
     const std::string base = partial_base(e, expect);
     SavedCkpt rec;
+    uint64_t saved;                                      // bytes in the .part: == rec.bytes, or more for a disk-backed stream's record
     {
         FILE *f = fopen((base + ".ckpt").c_str(), "rb");
         if (!f) return DM_ENOENT;
-        const bool got = fread(&rec, sizeof rec, 1, f) == 1;
+        SavedDiskCkpt any;
+        memset(&any, 0, sizeof any);
+        const size_t got = fread(&any, 1, sizeof any, f);
         fclose(f);
-        if (!got || memcmp(rec.magic, kCkptMagic, 8) != 0 || rec.abi != DM_ABI_VERSION || (rec.bytes & 63) ||
+        rec = any.ck;
+        const bool v2 = got == sizeof(SavedCkpt) && memcmp(rec.magic, kCkptMagic, 8) == 0;
+        const bool v3 = got == sizeof(SavedDiskCkpt) && memcmp(rec.magic, kDiskCkptMagic, 8) == 0;
+        saved = v3 ? any.saved : rec.bytes;
+        if (!(v2 || v3) || rec.abi != DM_ABI_VERSION || (rec.bytes & 63) || (saved & 63) || saved < rec.bytes ||
             memcmp(rec.expect, expect, 32) != 0) {
             unlink((base + ".ckpt").c_str()); unlink((base + ".part").c_str());
             if (e->n_suspended) e->n_suspended--;
@@ -735,17 +882,43 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
     ck.bytes = rec.bytes; ck.abi = DM_ABI_VERSION;
     int rc = stream_resume_impl(e, &ck, expect, size_hint ? size_hint : rec.size_hint, id);
     if (rc != DM_OK) return rc;
-    // Re-supply the saved prefix (cached, not re-hashed) through the ordinary range path: ring -> DMA -> extent.
-    // A blob too large for the arena continues verify-only: it retains nothing, so there is no prefix to load.
-    bool retains = true;
-    if (auto sp = find_stream(e, *id)) { std::lock_guard<std::mutex> g(sp->mu); retains = !sp->verify_only; }
-    int fd = rec.bytes && retains ? open((base + ".part").c_str(), O_RDONLY) : -1;
-    bool ok = rec.bytes == 0 || !retains || fd >= 0;
-    if (ok && rec.bytes && retains) {
+    // Re-supply the saved prefix [0, rec.bytes) (cached, not re-hashed) and the saved bytes past it (hashed) through
+    // the ordinary range path: ring -> DMA -> extent, or ring -> file.  A blob too large for the arena continues
+    // verify-only: it retains nothing, so only the bytes still to be hashed are loaded.  A disk-backed stream
+    // resuming a disk-backed record adopts the saved file instead: renamed back, nothing copied.
+    bool retains = true, adopted = false;
+    if (auto sp = find_stream(e, *id)) {
+        std::lock_guard<std::mutex> g(sp->mu);
+        Stream *s = sp.get();
+        retains = !s->verify_only || s->disk;
+        if (s->disk && saved) {
+            close(s->fd);
+            s->fd = -1;
+            bool moved = rename((base + ".part").c_str(), s->path.c_str()) == 0;
+            if (moved) s->fd = open(s->path.c_str(), O_RDWR | O_CLOEXEC);
+            if (moved && s->fd < 0) {                    // adopted but not openable: give the saved bytes back untouched
+                if (rename(s->path.c_str(), (base + ".part").c_str()) != 0) s->path.clear();   // (then never unlinked)
+                moved = false;
+            }
+            // not adopted: a fresh file of the stream's own, the saved bytes are loaded into it below
+            if (!moved && !s->path.empty()) s->fd = open(s->path.c_str(), O_CREAT | O_TRUNC | O_RDWR | O_CLOEXEC, 0644);
+            if (moved) {
+                adopted = true;
+                add_interval(s->written, 0, saved);
+                if (rec.bytes) add_interval(s->prefix_cover, 0, rec.bytes);
+                s->dma_issued = s->landed = s->received = saved;
+                disk_feed(e, sp);
+            }
+        }
+    }
+    const uint64_t from = retains ? 0 : rec.bytes;
+    int fd = saved > from && !adopted ? open((base + ".part").c_str(), O_RDONLY) : -1;
+    bool ok = adopted || saved == from || fd >= 0;
+    if (ok && !adopted && saved > from) {
         std::vector<uint8_t> buf(1u << 20);
-        uint64_t off = 0;
-        while (ok && off < rec.bytes) {
-            const size_t want = (size_t)std::min<uint64_t>(buf.size(), rec.bytes - off);
+        uint64_t off = from;
+        while (ok && off < saved) {
+            const size_t want = (size_t)std::min<uint64_t>(buf.size(), saved - off);
             const ssize_t got = pread(fd, buf.data(), want, (off_t)off);
             if (got < 0 && errno == EINTR) continue;
             if (got <= 0) { ok = false; break; }
@@ -763,7 +936,7 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
     unlink((base + ".ckpt").c_str());                    // the stream owns the download again
     unlink((base + ".part").c_str());
     if (e->n_suspended) e->n_suspended--;
-    if (resume_from) *resume_from = rec.bytes;
+    if (resume_from) *resume_from = saved;
     return DM_OK;
 }
 
@@ -844,6 +1017,7 @@ static int begin_finish(dm_engine *e, const std::shared_ptr<Stream> &sp, std::un
     if (!s->islands.empty()) return fail(DM_ESTATE, "blob has holes: ranges missing before the last byte");
     if (s->lost != DM_OK) return fail(s->lost, kLostText);      // the pump may have recalled (and lost) a slab while take_slab waited
     s->st = St::Finishing;
+    disk_feed(e, sp);                                  // a disk-backed body's last partial block may be read back now
     mark_dirty(e, sp, nullptr);
     return DM_OK;
 }
@@ -865,6 +1039,7 @@ static int stream_finish_impl(dm_engine *e, uint64_t id, uint8_t digest_out[32],
     Stream *s = sp.get();
     std::shared_ptr<Blob> blob;
     bool failed = false;
+    int disk_rc = DM_OK;
     {
         std::unique_lock<std::mutex> g(s->mu);
         int rc = begin_finish(e, sp, g);
@@ -877,9 +1052,11 @@ static int stream_finish_impl(dm_engine *e, uint64_t id, uint8_t digest_out[32],
         if (matched) *matched = s->matched;
         blob = s->blob;
         failed = s->cuda_failed;
+        if (s->disk) disk_rc = s->lost;
     }
     drop_stream(e, sp, true);
     if (failed) return fail(DM_ECUDA, "a CUDA copy or launch failed while this stream was being hashed; nothing was cached");
+    if (disk_rc != DM_OK) return fail(disk_rc, "the disk-backed stream's file could not be written or published; nothing was cached");
     if (blob && (e->cfg.flags & DM_F_DISK_SYNC) && !e->cas_dir.empty()) {
         std::unique_lock<std::mutex> g(e->spill_mu);
         e->spill_done_cv.wait(g, [&] { std::lock_guard<std::mutex> g2(e->mu); return blob->spill_done; });
@@ -895,23 +1072,35 @@ static int stream_abort_impl(dm_engine *e, uint64_t id)
     auto sp = find_stream(e, id);
     if (!sp) return fail(DM_EINVAL, "unknown stream id");
     Stream *s = sp.get();
-    bool free_now;
+    bool free_now = false;
     {
-        std::lock_guard<std::mutex> g(s->mu);
+        std::unique_lock<std::mutex> g(s->mu);
         if (s->st == St::Done || s->st == St::Aborted) return fail(DM_ESTATE, "stream already closed");
         if (s->cur) { slab_put(e, s->cur); s->cur = nullptr; s->cur_fill = 0; }
         s->carry_fill = 0;
         s->small.reset(); s->small_fill = 0; s->small_cap = 0;
         for (Stream::Part &pt : s->parts) slab_put(e, pt.slab);
         s->parts.clear();
+        if (s->disk) {
+            // writes and read-backs in flight use the file and ring slabs (a read-back of an aborted stream returns
+            // its slab itself), and a publication may be renaming the file: let them end first.  Who releases the
+            // slot is decided here, where the state changes: the pump's reap sees Aborted as soon as it is set.
+            s->st = St::Aborted;
+            free_now = s->jobs_inflight == 0;
+            s->cv.wait(g, [&] { return s->disk_writes == 0 && s->disk_reads == 0 && !s->publishing; });
+            if (s->fd >= 0) { close(s->fd); s->fd = -1; }
+            if (!s->path.empty()) unlink(s->path.c_str());
+        }
         if (!s->staged.empty()) {            // their DMAs may be in flight: drain before the ring reuses them
             cudaSetDevice(e->device);
             cudaStreamSynchronize(e->copy_stream[s->id % kCopyStreams]);
             for (auto &ps : s->staged) slab_return(e, ps.first);
             s->staged.clear();
         }
-        s->st = St::Aborted;
-        free_now = s->jobs_inflight == 0;
+        if (!s->disk) {
+            s->st = St::Aborted;
+            free_now = s->jobs_inflight == 0;
+        }
         if (free_now) pack_release_member(e, s);         // (a job already built keeps the pack until it is reaped)
     }
     if (free_now) {

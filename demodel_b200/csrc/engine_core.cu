@@ -246,6 +246,10 @@ void slab_put(dm_engine *e, Slab *s)
         e->slab_free.push_back(s);
     }
     e->slab_cv.notify_one();
+    if (e->feed_starved.load(std::memory_order_relaxed)) {        // a disk-backed read-back waits for a slab
+        { std::lock_guard<std::mutex> g(e->disk_mu); e->feed_kick = true; }
+        e->disk_cv.notify_one();
+    }
 }
 
 void slab_return(dm_engine *e, Slab *s)
@@ -339,6 +343,12 @@ int submit_slab(dm_engine *e, const std::shared_ptr<Stream> &sp)
     s->cur = nullptr; s->cur_fill = 0;
     if (n == 0) { slab_put(e, slab); return DM_OK; }
     e->st_ingested.fetch_add(n, std::memory_order_relaxed);       // per slab, not per write: one shared line, many writer threads
+    if (s->disk) {
+        disk_write(e, sp, slab, s->dma_issued, n);
+        s->dma_issued += n;
+        absorb_islands(s);
+        return DM_OK;
+    }
     if (s->verify_only) {
         cudaSetDevice(e->device);
         cudaError_t err = cudaMemcpyAsync(slab->dev, slab->host, n, cudaMemcpyHostToDevice, e->copy_stream[s->id % kCopyStreams]);
@@ -369,11 +379,15 @@ int submit_part(dm_engine *e, const std::shared_ptr<Stream> &sp, size_t idx)
     s->range_mode = true;
     if (pt.fill == 0) { slab_put(e, pt.slab); return DM_OK; }
     e->st_ingested.fetch_add(pt.fill, std::memory_order_relaxed);
-    int rc = dma_range(e, sp, pt.slab, pt.base, pt.fill);
-    if (rc != DM_OK) return s->lost = rc;
+    if (s->disk) disk_write(e, sp, pt.slab, pt.base, pt.fill);
+    else {
+        int rc = dma_range(e, sp, pt.slab, pt.base, pt.fill);
+        if (rc != DM_OK) return s->lost = rc;
+    }
     if (pt.base + pt.fill <= s->resume_base) add_interval(s->prefix_cover, pt.base, pt.base + pt.fill);
     else add_interval(s->islands, pt.base, pt.base + pt.fill);
     absorb_islands(s);
+    if (s->disk) return DM_OK;                  // the slab comes back from the disk thread
     mark_dirty(e, sp, pt.slab);
     if (s->followers) s->cv.notify_all();
     return DM_OK;
@@ -646,6 +660,12 @@ void complete_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, const uint
     ext.swap(s->extents);
     s->capacity = 0;
     const uint64_t size = s->dma_issued;
+    if (s->disk) {                              // the rename into the disk tier runs on a disk thread, finish waits for it
+        s->publishing = true;
+        g.unlock();
+        disk_enqueue(e, DiskTask{DiskTask::Publish, sp});
+        return;
+    }
     const Digest d = s->digest;
     const int matched = s->matched;
     // a resumed stream is cacheable only if the already-hashed prefix was re-supplied
@@ -707,6 +727,7 @@ void reap_cycle(dm_engine *e, Cycle &c)
                 pack_release_member(e, sp.get());
             }
             sp->jobs_inflight--;
+            if (sp->disk) disk_feed(e, sp);                        // a staged slab was used up: read the next one back
             free_now = sp->st == St::Aborted && sp->jobs_inflight == 0;
             wake = sp->ckpt_waiter;
         }
@@ -768,7 +789,7 @@ bool run_cycle(dm_engine *e, Cycle &c, std::vector<std::shared_ptr<Stream>> &rea
     for (auto &sp : ready) {
         Stream *s = sp.get();
         std::lock_guard<std::mutex> g(s->mu);
-        if (s->st == St::Aborted || s->st == St::Done || s->final_issued) { s->queued = false; continue; }
+        if (s->st == St::Aborted || s->st == St::Done || s->final_issued || s->suspending) { s->queued = false; continue; }
         // one job per stream in flight: its next job chains on the state this one writes
         if (s->jobs_inflight || c.njobs >= e->max_jobs) { again.push_back(sp); continue; }
         const bool finishing = s->st == St::Finishing;
@@ -809,9 +830,9 @@ bool run_cycle(dm_engine *e, Cycle &c, std::vector<std::shared_ptr<Stream>> &rea
                 n = s->staged.front().second;               // whole slab; only the last may hold a partial block
                 src = job_slab->dev;
                 s->staged.pop_front();
-                final = finishing && s->staged.empty();
+                final = finishing && s->staged.empty() && (!s->disk || disk_fed(s));
                 if (!final && (n & 63)) { final = false; }   // cannot happen: mid-stream slabs are full
-            } else if (!finishing) { s->queued = false; continue; }
+            } else if (!finishing || (s->disk && !disk_fed(s))) { s->queued = false; continue; }   // (a read-back re-queues it)
             else n = 0;
         } else {
             src = n ? seg_at(e, s->extents, s->hash_issued, &contig) : nullptr;
@@ -913,7 +934,7 @@ void flush_partial_slabs(dm_engine *e)
         for (size_t i = s->parts.size(); i-- > 0;)
             if (s->parts[i].fill) lose(submit_part(e, sp, i));
         if (!s->cur || s->cur_fill == 0) continue;
-        if (s->verify_only && (s->cur_fill & 63)) {              // slab-by-slab hashing needs whole blocks:
+        if (s->verify_only && !s->disk && (s->cur_fill & 63)) {  // slab-by-slab hashing needs whole blocks:
             const uint32_t whole = s->cur_fill & ~63u;           // send those, keep the tail in the stream
             s->carry_fill = s->cur_fill - whole;
             memcpy(s->carry, s->cur->host + whole, s->carry_fill);
@@ -969,7 +990,7 @@ void pump_main(dm_engine *e)
         // is repeated every 16 passes while the writers are still waiting and still nothing is in flight.
         {
             const bool asked = e->ring_starved.exchange(false);
-            if (e->ring_waiters.load() > 0 && e->slabs_returning.load() == 0) {
+            if ((e->ring_waiters.load() > 0 || e->feed_starved.load()) && e->slabs_returning.load() == 0) {
                 if (asked || ++starve_ticks >= 16) { starve_ticks = 0; flush_partial_slabs(e); }
             } else starve_ticks = asked ? 15 : 0;      // re-check on the very next pass if somebody just asked
         }
@@ -988,7 +1009,7 @@ void pump_main(dm_engine *e)
             std::unique_lock<std::mutex> g(e->work_mu);
             const bool idle = !n_inflight && !b_live && ready.empty() && slabs.empty() && live_packs.empty();
             if (e->dirty.empty() && e->pending_slabs.empty() && !e->stop && !launched && !reaped && !landed_any) {
-                if (idle && e->ring_waiters.load() == 0)
+                if (idle && e->ring_waiters.load() == 0 && !e->feed_starved.load())
                     e->work_cv.wait(g, [&] { return !e->dirty.empty() || !e->pending_slabs.empty() || e->stop || e->ring_starved.load(); });
                 else e->work_cv.wait_for(g, std::chrono::microseconds(40));
             }
@@ -1184,6 +1205,218 @@ int ensure_dev_ring(dm_engine *e)
     CU_TRY(cudaMalloc(&e->dev_ring, bytes));
     for (size_t i = 0; i < e->slab_store.size(); ++i) e->slab_store[i].dev = e->dev_ring + i * e->cfg.slab_bytes;
     return DM_OK;
+}
+
+// ---- disk-backed streams (DM_F_DISK_DIRECT) ------------------------------------------
+// The client writes into ring slabs as on every stream; a full slab (or a recalled partial one, or a range part)
+// is pwritten at its blob offset by a disk thread and returns to the ring when the write completes, so the
+// client runs at the speed of the network and the disk.  The hash follows from the file: a disk thread reads
+// the contiguous written prefix back into a ring slab, copies it to the slab's device mirror and stages it,
+// and the pump hashes it exactly as a verify-only slab (one slab per job).  The digest is therefore over the
+// bytes of the file that gets published.
+
+std::string incoming_path(const dm_engine *e, uint64_t id)
+{
+    return e->cas_dir + "/incoming/" + std::to_string((long)getpid()) + "-" + std::to_string(e->device) + "-" +
+           std::to_string(id) + ".part";
+}
+
+void disk_enqueue(dm_engine *e, DiskTask t)
+{
+    { std::lock_guard<std::mutex> g(e->disk_mu); e->disk_q.push_back(std::move(t)); }
+    e->disk_cv.notify_one();
+}
+
+void disk_write(dm_engine *e, const std::shared_ptr<Stream> &sp, Slab *slab, uint64_t off, uint32_t n)
+{
+    e->slabs_returning.fetch_add(1, std::memory_order_relaxed);     // comes back by itself once written
+    sp->disk_writes++;
+    disk_enqueue(e, DiskTask{DiskTask::Write, sp, slab, sp->fd, off, n});
+}
+
+bool disk_fed(const Stream *s)
+{
+    return s->disk_writes == 0 && s->disk_reads == 0 &&
+           (s->staged_to == s->dma_issued || s->lost != DM_OK || s->cuda_failed);
+}
+
+void disk_feed(dm_engine *e, const std::shared_ptr<Stream> &sp)
+{
+    Stream *s = sp.get();
+    // at most two slabs on the hash side per stream, counting the one its running job reads: with the writer's slab
+    // a disk-backed body never holds more than three
+    if (!s->disk || s->disk_reads || s->staged.size() + s->jobs_inflight >= 2 || s->suspending || s->lost != DM_OK ||
+        s->cuda_failed)
+        return;
+    if (s->st != St::Open && s->st != St::Finishing) return;
+    uint64_t end = s->staged_to;
+    auto it = s->written.upper_bound(s->staged_to);
+    if (it != s->written.begin() && std::prev(it)->second > s->staged_to) end = std::prev(it)->second;
+    uint64_t n = std::min<uint64_t>(end - s->staged_to, e->cfg.slab_bytes);
+    // whole blocks only (jobs chain block by block); the final partial block once nothing more can arrive
+    const bool last = s->st == St::Finishing && s->disk_writes == 0 && s->staged_to + n == s->dma_issued;
+    if (!last) n &= ~63ull;
+    if (n == 0) return;
+    Slab *sl = slab_try_get(e);
+    if (!sl) {
+        { std::lock_guard<std::mutex> g(e->disk_mu); e->disk_starved.push_back(sp); e->feed_starved.store(true); }
+        { std::lock_guard<std::mutex> g(e->work_mu); e->ring_starved.store(true); }     // the pump may recall partial slabs
+        e->work_cv.notify_one();
+        e->disk_cv.notify_one();
+        return;
+    }
+    e->slabs_returning.fetch_add(1, std::memory_order_relaxed);     // staged: back to the ring when its job is reaped
+    s->disk_reads++;
+    disk_enqueue(e, DiskTask{DiskTask::Read, sp, sl, s->fd, s->staged_to, (uint32_t)n});
+    s->staged_to += n;
+}
+
+static int pwrite_all(int fd, const uint8_t *p, uint64_t n, uint64_t off)
+{
+    while (n) {
+        const ssize_t r = pwrite(fd, p, n, (off_t)off);
+        if (r < 0 && errno == EINTR) continue;
+        if (r <= 0) return r < 0 ? errno : ENOSPC;
+        p += r; n -= (uint64_t)r; off += (uint64_t)r;
+    }
+    return 0;
+}
+
+static bool pread_all(int fd, uint8_t *p, uint64_t n, uint64_t off)
+{
+    while (n) {
+        const ssize_t r = pread(fd, p, n, (off_t)off);
+        if (r < 0 && errno == EINTR) continue;
+        if (r <= 0) return false;
+        p += r; n -= (uint64_t)r; off += (uint64_t)r;
+    }
+    return true;
+}
+
+static void disk_task_write(dm_engine *e, DiskTask &t)
+{
+    Stream *s = t.sp.get();
+    const int err = pwrite_all(t.fd, t.slab->host, t.n, t.off);
+    slab_return(e, t.slab);
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (err && s->lost == DM_OK) s->lost = fail(DM_EIO, "write to the disk-backed stream's file failed");
+        if (!err) add_interval(s->written, t.off, t.off + t.n);
+        s->disk_writes--;
+        disk_feed(e, t.sp);
+        if (s->st == St::Finishing) mark_dirty(e, t.sp, nullptr);   // a failed write still has to end in a (failed) verdict
+    }
+    s->cv.notify_all();
+}
+
+static void disk_task_read(dm_engine *e, DiskTask &t)
+{
+    Stream *s = t.sp.get();
+    cudaStream_t cs = e->copy_stream[s->id % kCopyStreams];
+    const bool got = pread_all(t.fd, t.slab->host, t.n, t.off);
+    const cudaError_t err = got ? cudaMemcpyAsync(t.slab->dev, t.slab->host, t.n, cudaMemcpyHostToDevice, cs) : cudaSuccess;
+    if (err != cudaSuccess) (void)cudaGetLastError();
+    bool keep;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        s->disk_reads--;
+        if (!got && s->lost == DM_OK) s->lost = fail(DM_EIO, "read-back of the disk-backed stream's file failed");
+        if (err != cudaSuccess) s->cuda_failed = true;
+        keep = got && err == cudaSuccess && s->st != St::Aborted && !s->suspending;
+        if (keep) {
+            e->st_h2d += t.n;
+            s->staged.emplace_back(t.slab, t.n);
+            disk_feed(e, t.sp);
+        }
+        if (keep || s->st == St::Finishing) mark_dirty(e, t.sp, nullptr);
+    }
+    if (!keep) {
+        cudaStreamSynchronize(cs);               // the copy out of the slab may still be running
+        slab_return(e, t.slab);
+    }
+    s->cv.notify_all();
+}
+
+// The final job has been reaped.  Matched and whole: the file becomes the blob in the disk tier; anything else
+// (a mismatch, a failed copy or launch, a lost write, an abort): the file is removed.
+static void disk_task_publish(dm_engine *e, DiskTask &t)
+{
+    Stream *s = t.sp.get();
+    std::unique_lock<std::mutex> g(s->mu);
+    const bool whole = s->resume_base == 0 ||
+                       (s->prefix_cover.size() == 1 && s->prefix_cover.begin()->first == 0 &&
+                        s->prefix_cover.begin()->second >= s->resume_base);
+    const bool keep = s->st != St::Aborted && s->matched && whole && s->lost == DM_OK && !s->cuda_failed;
+    const int fd = s->fd;
+    s->fd = -1;
+    const std::string path = s->path;
+    const uint64_t size = s->dma_issued;
+    auto b = std::make_shared<Blob>();
+    b->digest = s->digest; b->size = size;
+    b->meta.swap(s->meta);
+    const bool counted_mismatch = !s->matched;
+    g.unlock();
+    bool ok = keep && ftruncate(fd, (off_t)size) == 0 && (!(e->cfg.flags & DM_F_DISK_SYNC) || fsync(fd) == 0);
+    if (fd >= 0) close(fd);
+    std::shared_ptr<Blob> pub;
+    if (ok) {
+        const std::string dst = blob_path(e, b->digest.b);
+        mkdirs(dst);
+        struct stat st;
+        const bool had = stat(dst.c_str(), &st) == 0;          // already in the disk tier: keep that copy
+        if (had) unlink(path.c_str());
+        else ok = rename(path.c_str(), dst.c_str()) == 0;
+        if (ok && !had) write_sidecar(dst + ".meta", *b);
+    }
+    if (ok) {
+        std::lock_guard<std::mutex> gi(e->mu);
+        auto it = e->blobs.find(b->digest);
+        if (it != e->blobs.end()) pub = it->second;
+        else {
+            b->on_disk = b->spill_done = true;
+            e->blobs[b->digest] = b;
+            pub = b;
+        }
+        if (!pub->on_disk) { pub->on_disk = true; pub->spill_done = true; }
+    }
+    if (!ok) unlink(path.c_str());
+    if (ok) e->st_committed++;
+    else if (counted_mismatch || keep) e->st_mismatch++;
+    g.lock();
+    if (keep && !ok) { s->matched = 0; if (s->lost == DM_OK) s->lost = fail(DM_EIO, "could not move the verified file into the disk tier"); }
+    s->publishing = false;
+    s->blob = pub;
+    if (s->st != St::Aborted) s->st = St::Done;
+    g.unlock();
+    s->cv.notify_all();
+}
+
+void disk_main(dm_engine *e)
+{
+    cudaSetDevice(e->device);
+    for (;;) {
+        DiskTask t;
+        std::vector<std::weak_ptr<Stream>> retry;
+        {
+            std::unique_lock<std::mutex> g(e->disk_mu);
+            // A starved read-back may be queued by any thread (the pump's reap, a finishing client, resume) while every
+            // disk thread sleeps: it is work of its own, retried at once, then whenever a slab is put back (slab_put
+            // notifies) and at least every millisecond while the ring stays empty.
+            auto work = [&] { return !e->disk_q.empty() || e->disk_stop; };
+            if (e->disk_starved.empty()) e->disk_cv.wait(g, [&] { return work() || !e->disk_starved.empty(); });
+            else e->disk_cv.wait_for(g, std::chrono::milliseconds(1), [&] { return work() || e->feed_kick; });
+            e->feed_kick = false;
+            if (e->disk_q.empty() && e->disk_stop) break;
+            if (!e->disk_starved.empty()) { retry.swap(e->disk_starved); e->feed_starved.store(false); }
+            if (!e->disk_q.empty()) { t = std::move(e->disk_q.front()); e->disk_q.pop_front(); }
+        }
+        for (auto &w : retry)
+            if (auto sp = w.lock()) { std::lock_guard<std::mutex> g(sp->mu); disk_feed(e, sp); }
+        if (!t.sp) continue;
+        if (t.kind == DiskTask::Write) disk_task_write(e, t);
+        else if (t.kind == DiskTask::Read) disk_task_read(e, t);
+        else disk_task_publish(e, t);
+    }
 }
 
 std::shared_ptr<Stream> find_stream(dm_engine *e, uint64_t id)

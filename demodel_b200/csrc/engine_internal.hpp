@@ -70,6 +70,7 @@ constexpr int kIngestMaxChunks = 8;
 constexpr uint32_t kIngestChunkMin = 16384;  // jobs per chunk at least: 512 warps of the lane-per-stream kernel
 constexpr int kCompleters = 2;             // threads that compare / publish finished bodies, so the pump only launches and reaps
 constexpr int kBounceReserve = 2 * kSpillThreads + 2;          // never lent to windows: the spill thread and one-shot reads need some
+constexpr int kDiskThreads = 4;            // DM_F_DISK_DIRECT: file writes, read-backs and publications of disk-backed streams
 
 inline uint64_t round_up(uint64_t x, uint64_t a) { return (x + a - 1) / a * a; }
 
@@ -175,6 +176,18 @@ struct Stream {
     uint8_t carry[64];
     uint32_t carry_fill = 0;
     std::deque<std::pair<Slab *, uint32_t>> staged;
+    // Disk-backed streams (DM_F_DISK_DIRECT): a verify-only stream whose bytes are kept in a file of their own,
+    // <cas_dir>/incoming/<pid>-<device>-<id>.part.  Every slab and range part is written there by a disk thread
+    // and goes back to the ring when the write completes; the hash reads the bytes back from the file, in order,
+    // into `staged` (whole blocks, at most two slabs ahead).  The verified file is renamed into the disk tier.
+    bool disk = false;
+    int fd = -1;
+    std::string path;
+    std::map<uint64_t, uint64_t> written;        // [start, end) whose pwrite has completed
+    uint64_t staged_to = 0;                      // bytes read back for hashing (from resume_base on)
+    uint32_t disk_writes = 0, disk_reads = 0;    // in flight on the disk threads (at most one read)
+    bool publishing = false;                     // the final rename / sidecar is running on a disk thread
+    bool suspending = false;                     // dm_stream_suspend: no further read-back or launch
     // A body announced (Content-Length) as at most tiny_max bytes never takes a ring slab: its bytes gather in this
     // private buffer and go straight into a pack when it finishes.  Anything that needs a real slab (more bytes than
     // announced, range parts, zero-copy windows, checkpoints) moves them into one first (take_slab).
@@ -243,6 +256,18 @@ struct SlabBatch {
 };
 
 struct Bounce { uint8_t *host = nullptr; cudaStream_t stream{}; };
+
+// Work for the disk threads of DM_F_DISK_DIRECT.  Write: `slab` holds `n` bytes for blob offset `off`.
+// Read: `slab` receives [off, off + n) of the file and is staged for hashing.  Publish: the final job has been
+// reaped, the verdict is in the stream.
+struct DiskTask {
+    enum Kind { Write, Read, Publish } kind = Write;
+    std::shared_ptr<Stream> sp;
+    Slab *slab = nullptr;
+    int fd = -1;
+    uint64_t off = 0;
+    uint32_t n = 0;
+};
 
 }  // namespace dmi
 
@@ -323,6 +348,15 @@ struct dm_engine {
     std::condition_variable spill_cv, spill_done_cv;
     std::deque<std::shared_ptr<Blob>> spill_q;
     std::vector<std::thread> spillers;   // kSpillThreads writers of the disk tier
+
+    std::mutex disk_mu;                  // DM_F_DISK_DIRECT: the disk threads' queue (taken after a stream mutex, never before)
+    std::condition_variable disk_cv;
+    std::deque<DiskTask> disk_q;
+    std::vector<std::weak_ptr<Stream>> disk_starved;   // read-backs that found the ring empty: retried by the disk threads
+    std::atomic<bool> feed_starved{false};             // ... and the pump recalls partly filled slabs for them
+    bool feed_kick = false;                            // a slab was put back while read-backs were starved (disk_mu)
+    bool disk_stop = false;
+    std::vector<std::thread> disk_threads;
 
     std::mutex bounce_mu;
     std::condition_variable bounce_cv;
@@ -443,6 +477,12 @@ bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int 
 bool spill_one(dm_engine *e, Blob *b);
 void spill_main(dm_engine *e);
 int ensure_dev_ring(dm_engine *e);
+std::string incoming_path(const dm_engine *e, uint64_t id);
+void disk_enqueue(dm_engine *e, DiskTask t);
+void disk_write(dm_engine *e, const std::shared_ptr<Stream> &sp, Slab *slab, uint64_t off, uint32_t n);   // stream mutex held
+void disk_feed(dm_engine *e, const std::shared_ptr<Stream> &sp);   // stream mutex held: start the next read-back if one is due
+bool disk_fed(const Stream *s);               // stream mutex held: every byte is written and staged (or never will be)
+void disk_main(dm_engine *e);
 std::shared_ptr<Stream> find_stream(dm_engine *e, uint64_t id);
 void drop_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, bool release_slot);
 int ensure_ingest_scratch(dm_engine *e, uint32_t n);

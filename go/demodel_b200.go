@@ -59,6 +59,7 @@ type Config struct {
 	MaxStreams    uint32 // 0 = 65536
 	CacheDir      string // "" = HBM tier only
 	DiskSync      bool
+	DiskDirect    bool // bodies too large for HBM (all bodies when HBM holds none) are cached on disk; needs CacheDir
 }
 
 // Pool owns one engine per GPU and routes blobs by digest prefix
@@ -92,6 +93,9 @@ func Open(cfg Config) (*Pool, error) {
 		c.cas_dir = dir
 		if cfg.DiskSync {
 			c.flags |= C.DM_F_DISK_SYNC
+		}
+		if cfg.DiskDirect {
+			c.flags |= C.DM_F_DISK_DIRECT
 		}
 		var e *C.dm_engine
 		if err := check(nil, 0, C.dm_engine_create(&c, &e)); err != nil {

@@ -60,6 +60,12 @@ typedef struct dm_engine dm_engine;   /* opaque; owned by caller between create/
 #define DM_F_DISK_SYNC    0x2u  /* dm_stream_finish returns only after the disk tier holds the blob */
 #define DM_F_NUMA_LOCAL   0x4u  /* pin the ring / bounce buffers and start the engine's threads on the NUMA node the
                                   * GPU hangs off (sysfs); silently skipped when the topology is not visible */
+#define DM_F_DISK_DIRECT  0x8u  /* needs cas_dir (else dm_engine_create: DM_EINVAL).  A stream that would be verify-only
+                                  * (size_hint > hbm_cas_bytes, or every stream under DM_F_NO_HBM_CAS) is DISK-BACKED
+                                  * instead: its bytes are written to <cas_dir>/incoming/ as they arrive, each ring slab
+                                  * returns as soon as its write completes, the GPU hashes the bytes read back from that
+                                  * file, and the verified file is renamed into the disk tier.  Range parts, suspend and
+                                  * resume work as on HBM streams; followers (dm_cache_follow) do not attach to them. */
 
 typedef struct dm_config {
     uint32_t struct_size;     /* = sizeof(dm_config); ABI guard */
@@ -141,7 +147,10 @@ int dm_stream_write(dm_engine *e, uint64_t id, const void *buf, size_t len);
  * Ollama fetch one large blob as parallel `Range` requests).  The bytes land
  * at their place in the blob's HBM extent at once; the digest advances over the
  * contiguous prefix as it grows.  Ranges must not overlap; up to 64 parts may
- * be open on one stream.  dm_stream_finish fails with DM_ESTATE while holes remain. */
+ * be open on one stream.  dm_stream_finish fails with DM_ESTATE while holes remain.
+ * Disk-backed streams (DM_F_DISK_DIRECT) accept parts too: they are written at their offset in the stream's
+ * file, and the hash reads the contiguous prefix back from there.  A failed file write (disk full, file size
+ * limit, I/O error) makes every later call on the stream return DM_EIO; nothing is published. */
 int dm_stream_write_at(dm_engine *e, uint64_t id, uint64_t offset, const void *buf, size_t len);
 
 /* Mid-state checkpoint / resume of an interrupted download (SURVEY.md §8f-3).
@@ -149,7 +158,9 @@ int dm_stream_write_at(dm_engine *e, uint64_t id, uint64_t offset, const void *b
  * hashed and returns (state words, byte count).  dm_stream_resume opens a new
  * stream that continues from such a checkpoint: bytes from `ck->bytes` on are
  * hashed; the prefix may be re-supplied with dm_stream_write_at purely for
- * caching — if it is not, the blob is verified but not published in the CAS. */
+ * caching — if it is not, the blob is verified but not published in the CAS.
+ * On a disk-backed stream (DM_F_DISK_DIRECT) the hash trails the client by the hash rate (one stream: tens of
+ * MB/s), so dm_stream_checkpoint, which waits for every in-order block, can take minutes on a large body. */
 typedef struct dm_checkpoint {
     uint32_t h[8];      /* SHA-256 chaining value after `bytes` bytes */
     uint64_t bytes;     /* multiple of 64 */
@@ -167,7 +178,12 @@ int dm_stream_resume(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect
  * dm_stream_resume_saved - in this process or after dm_engine_create over the same cas_dir - opens a stream
  * that continues from the saved state: the saved prefix is loaded back into the blob's HBM extent (so the
  * finished blob is cached whole) and only the bytes from *resume_from on are hashed.  DM_ENOENT when
- * nothing is saved for `expect`.  The saved files are removed once a resumed stream has taken them over. */
+ * nothing is saved for `expect`.  The saved files are removed once a resumed stream has taken them over.
+ * Disk-backed streams (DM_F_DISK_DIRECT): suspend does not wait for the hash and copies nothing.  It saves the
+ * mid-state at the hashed position H, cuts the stream's file to the contiguous written prefix rounded down to 64
+ * (C >= H) and renames it to <hex>.part; *resume_from = C.  dm_stream_resume_saved hashes [H, C) from the saved
+ * file - a disk-backed stream adopts the file by renaming it back, an engine that can now hold the blob in HBM
+ * loads it - and the client continues at C. */
 int dm_stream_suspend(dm_engine *e, uint64_t id, uint64_t *resume_from);
 int dm_stream_resume_saved(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, uint64_t *resume_from);
 
