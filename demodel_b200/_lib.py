@@ -12,8 +12,8 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdemodel_b200.so")
 
-DM_OK, DM_EINVAL, DM_ENOMEM, DM_ENOENT, DM_ECUDA, DM_ESTATE, DM_EIO, DM_ENODEV, DM_ERANGE = (
-    0, -1, -2, -3, -4, -5, -6, -7, -8)
+DM_OK, DM_EINVAL, DM_ENOMEM, DM_ENOENT, DM_ECUDA, DM_ESTATE, DM_EIO, DM_ENODEV, DM_ERANGE, DM_ECORRUPT = (
+    0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 
 DM_F_NO_HBM_CAS = 0x1
 DM_F_DISK_SYNC = 0x2
@@ -110,6 +110,7 @@ SIGNATURES = {
     "dm_cache_meta": (C.c_int, [_P, C.c_uint64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "dm_cache_close": (C.c_int, [_P, C.c_uint64]),
     "dm_cache_evict": (C.c_int, [_P, _P]),
+    "dm_cache_promote": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_follow": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_alias_put": (C.c_int, [_P, C.c_char_p, _P]),
     "dm_cache_alias_get": (C.c_int, [_P, C.c_char_p, _P]),

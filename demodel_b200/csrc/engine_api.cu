@@ -112,6 +112,7 @@ const char *dm_strerror(int err)
     case DM_EIO: return "disk tier I/O error";
     case DM_ENODEV: return "no usable CUDA device";
     case DM_ERANGE: return "offset beyond blob end";
+    case DM_ECORRUPT: return "disk tier copy does not hash to its name";
     default: return "unknown error";
     }
 }
@@ -1117,7 +1118,243 @@ static int stream_abort_impl(dm_engine *e, uint64_t id)
     return DM_OK;
 }
 
+// ---- promotion: disk tier -> HBM (dm_cache_promote) ------------------------------------
+// Each blob is an internal stream opened with expect = its digest and size_hint = its file size: the file is pread
+// into acquired ring windows, flushed, and the next file starts while the pump hashes it.  The blob is registered as
+// disk-only first, so publish() re-homes it into HBM without queueing a spill: the verified file keeps its inode.
+
+namespace {
+
+constexpr int kPromoteThreads = 4;        // loaders: reads of different files overlap
+// Tiny bodies are flushed this many at a time.  Their hash takes less time than reading the next file, so one by one
+// each would be a launch of its own; together they share a pack DMA and a launch.
+constexpr size_t kPromoteTinyBatch = 256;
+
+struct Promotion {
+    Digest d;
+    int32_t status = DM_ENOENT;
+    uint64_t stream = 0;                  // open: the verdict is still to be collected
+    bool tiny = false;                    // at most tiny_max bytes, written to the stream's private buffer, not flushed yet
+    struct stat seen{};                   // the file that was read (st_dev / st_ino)
+    std::shared_ptr<Blob> mine;           // the disk-only entry this promotion registered (none if one existed)
+};
+
+// The sidecar's top-level "size" (it precedes "headers", so the first match is it).
+bool sidecar_size(const std::string &j, uint64_t *size)
+{
+    const size_t p = j.find("\"size\":");
+    if (p == std::string::npos) return false;
+    const char *s = j.c_str() + p + 7;
+    char *end = nullptr;
+    *size = strtoull(s, &end, 10);
+    return end != s;
+}
+
+// The disk copy under the index entry of `d` is bad or unchecked: forget an entry that is not in HBM, and spill
+// one that a stream has re-homed into HBM meanwhile again, from its verified HBM copy.  `only`: touch the entry only
+// if it is this object.
+void forget_disk_copy(dm_engine *e, const Digest &d, const Blob *only)
+{
+    std::shared_ptr<Blob> respill;
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(d);
+        if (it == e->blobs.end() || (only && it->second.get() != only)) return;
+        if (!it->second->in_hbm) e->blobs.erase(it);
+        else if (it->second->on_disk) {
+            respill = it->second;
+            respill->on_disk = respill->spill_done = false;
+        }
+    }
+    if (respill) {
+        { std::lock_guard<std::mutex> g(e->spill_mu); e->spill_q.push_back(respill); }
+        e->spill_cv.notify_all();
+    }
+}
+
+// The disk copy that was read (`seen`) does not hash to its name.  Remove it and its sidecar only while the path still
+// names that file: one a spill or a disk-backed stream renamed into place meanwhile is verified and stays.
+void drop_corrupt(dm_engine *e, const Digest &d, const struct stat &seen)
+{
+    const std::string path = blob_path(e, d.b);
+    struct stat now;
+    const bool exists = stat(path.c_str(), &now) == 0;
+    const bool same = exists && now.st_dev == seen.st_dev && now.st_ino == seen.st_ino;
+    if (same) { unlink(path.c_str()); unlink((path + ".meta").c_str()); }
+    if (!exists || same) forget_disk_copy(e, d, nullptr);
+}
+
+// The promotion ended without a verdict on the file (no slot or room, a failed read, copy or launch): take back the
+// entry it registered, which carries the file's unverified size.
+void promote_undo(dm_engine *e, Promotion &p)
+{
+    if (p.mine) forget_disk_copy(e, p.d, p.mine.get());
+}
+
+// Start loading one blob.  Returns 1 with p.stream open (and flushed unless p.tiny), or the blob's final status.
+// `tiny_buf` holds tiny_max bytes: a tiny body is read there and written into its stream's private buffer, so that it
+// holds no ring slab while it waits for its batch's flush.  `may_open`: false when the call has no stream slot to spare.
+int promote_start(dm_engine *e, Promotion &p, uint8_t *tiny_buf, bool may_open)
+{
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(p.d);
+        if (it != e->blobs.end() && it->second->in_hbm) return DM_OK;
+    }
+    if (e->cas_dir.empty()) return DM_ENOENT;
+    const std::string path = blob_path(e, p.d.b);
+    const int fd = open(path.c_str(), O_RDONLY | O_CLOEXEC);
+    if (fd < 0) return errno == ENOENT ? DM_ENOENT : fail(DM_EIO, "could not open the disk tier file");
+    if (fstat(fd, &p.seen) != 0) { close(fd); return fail(DM_EIO, "could not stat the disk tier file"); }
+    const uint64_t size = (uint64_t)p.seen.st_size;
+    std::string side;
+    if (FILE *mf = fopen((path + ".meta").c_str(), "r")) {
+        char tmp[4096];
+        size_t k;
+        while ((k = fread(tmp, 1, sizeof tmp, mf)) > 0) side.append(tmp, k);
+        fclose(mf);
+    }
+    uint64_t claimed;
+    if (!side.empty() && sidecar_size(side, &claimed) && claimed != size) {
+        close(fd);
+        drop_corrupt(e, p.d, p.seen);
+        return fail(DM_ECORRUPT, "disk tier file is not the size its sidecar says");
+    }
+    // checked here: a stream with this size_hint would silently become verify-only or disk-backed
+    if (size > e->cfg.hbm_cas_bytes) { close(fd); return fail(DM_ENOMEM, "blob is larger than the HBM arena"); }
+    if (!may_open) { close(fd); return fail(DM_ENOMEM, "no stream slot to spare for a promotion"); }
+    uint64_t id = 0;
+    int rc = stream_open_impl(e, p.d.b, size, &id, false);
+    if (rc != DM_OK) { close(fd); return rc; }
+    bool in_hbm = false;                                 // a stream published it meanwhile
+    {
+        // registered before the verdict (publish() then re-homes it without a spill); taken back on every outcome
+        // that does not verify the file
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(p.d);
+        if (it != e->blobs.end() && it->second->in_hbm) in_hbm = true;
+        else if (it == e->blobs.end()) {
+            p.mine = std::make_shared<Blob>();
+            p.mine->digest = p.d; p.mine->size = size;
+            p.mine->on_disk = p.mine->spill_done = true;
+            p.mine->sidecar.swap(side);
+            e->blobs[p.d] = p.mine;
+        }
+    }
+    if (in_hbm) { close(fd); stream_abort_impl(e, id); return DM_OK; }
+    p.tiny = size <= e->tiny_max;
+    for (uint64_t off = 0; p.tiny && rc == DM_OK && off < size;) {
+        ssize_t got;
+        do got = pread(fd, tiny_buf + off, size - off, (off_t)off); while (got < 0 && errno == EINTR);
+        if (got <= 0) { rc = fail(DM_EIO, "could not read the disk tier file"); break; }
+        off += (uint64_t)got;
+        if (off == size) rc = stream_write_impl(e, id, tiny_buf, size);
+    }
+    for (uint64_t off = 0; !p.tiny && rc == DM_OK && off < size;) {
+        void *win = nullptr;
+        size_t cap = 0;
+        rc = stream_acquire_impl(e, id, &win, &cap);
+        if (rc != DM_OK) break;
+        const size_t want = (size_t)std::min<uint64_t>(cap, size - off);
+        ssize_t got;
+        do got = pread(fd, win, want, (off_t)off); while (got < 0 && errno == EINTR);
+        if (got <= 0) {                                  // a read error, or the file shrank while it was read
+            stream_commit_impl(e, id, 0);
+            rc = fail(DM_EIO, "could not read the disk tier file");
+            break;
+        }
+        rc = stream_commit_impl(e, id, (size_t)got);
+        off += (uint64_t)got;
+    }
+    close(fd);
+    if (rc == DM_OK && !p.tiny) rc = stream_flush_impl(e, id);
+    if (rc != DM_OK) { stream_abort_impl(e, id); promote_undo(e, p); return rc; }
+    p.stream = id;
+    return 1;
+}
+
+int promote_verdict(dm_engine *e, Promotion &p)
+{
+    uint8_t got[32];
+    int matched = 0;
+    const int rc = stream_finish_impl(e, p.stream, got, &matched);
+    if (rc != DM_OK) {
+        stream_abort_impl(e, p.stream);                  // (an id finish released just says so)
+        promote_undo(e, p);
+        return rc;
+    }
+    if (matched) return DM_OK;
+    drop_corrupt(e, p.d, p.seen);
+    return DM_ECORRUPT;
+}
+
+}  // namespace
+
+static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
+{
+    if (!e || (n && (!digests || !status_out))) return fail(DM_EINVAL, "null argument");
+    if (e->cfg.flags & DM_F_NO_HBM_CAS) return fail(DM_ESTATE, "the engine has no HBM tier (DM_F_NO_HBM_CAS)");
+    std::vector<Promotion> work;
+    std::vector<uint32_t> slot_of(n);
+    {
+        std::unordered_map<Digest, uint32_t, DigestHash> first;
+        for (uint32_t i = 0; i < n; ++i) {
+            Digest d;
+            memcpy(d.b, digests + 32ull * i, 32);
+            auto ins = first.emplace(d, (uint32_t)work.size());
+            if (ins.second) { work.emplace_back(); work.back().d = d; }
+            slot_of[i] = ins.first->second;
+        }
+    }
+    // At most half of the slots that are free and not spoken for by other running calls: 0 with one or none, which
+    // stays dm_stream_open's.
+    size_t budget;
+    {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        const size_t free = e->free_slots.size();
+        budget = free > e->promote_reserved ? (free - e->promote_reserved) / 2 : 0;
+        e->promote_reserved += budget;
+    }
+    const size_t nthreads = std::min<size_t>({(size_t)kPromoteThreads, work.size(), std::max<size_t>(budget, 1)});
+    const size_t per_thread = std::max<size_t>(1, budget / std::max<size_t>(nthreads, 1));
+    std::atomic<size_t> next{0};
+    auto loader = [&] {
+        cudaSetDevice(e->device);
+        std::vector<uint8_t> tiny_buf(e->tiny_max);
+        std::deque<Promotion *> open;                    // verdict not collected yet (oldest first)
+        std::vector<Promotion *> unflushed;              // tiny ones among them, flushed together
+        // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
+        auto flush = [&] { for (Promotion *p : unflushed) stream_flush_impl(e, p->stream); unflushed.clear(); };
+        for (size_t k; (k = next.fetch_add(1)) < work.size();) {
+            if (open.size() >= per_thread) {
+                flush();
+                open.front()->status = promote_verdict(e, *open.front());
+                open.pop_front();
+            }
+            Promotion &p = work[k];
+            const int rc = promote_start(e, p, tiny_buf.data(), budget > 0);
+            if (rc != 1) { p.status = rc; continue; }
+            open.push_back(&p);
+            if (p.tiny) unflushed.push_back(&p);
+            if (unflushed.size() >= kPromoteTinyBatch) flush();
+        }
+        flush();
+        for (Promotion *p : open) p->status = promote_verdict(e, *p);
+    };
+    std::vector<std::thread> th;
+    for (size_t t = 1; t < nthreads; ++t) th.emplace_back(loader);
+    if (nthreads) loader();
+    for (auto &t : th) t.join();
+    { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved -= budget; }
+    for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
+    return DM_OK;
+}
+
 // ---- exported wrappers: file the error text under the stream id (dm_error_detail) ----
+int dm_cache_promote(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
+{
+    return note_err(e, 0, cache_promote_impl(e, digests, n, status_out));
+}
 int dm_stream_suspend(dm_engine *e, uint64_t id, uint64_t *resume_from) { return note_err(e, id, stream_suspend_impl(e, id, resume_from)); }
 int dm_stream_resume_saved(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, uint64_t *resume_from)
 {

@@ -484,6 +484,7 @@ std::string json_quote(const std::string &v)
 // identity-encoded body, which is what HF LFS oids and OCI layer digests are defined on.
 std::string sidecar_json(const Blob &b)
 {
+    if (!b.sidecar.empty()) return b.sidecar;
     std::string o = "{\"digest\":\"sha256:" + hex_of(b.digest.b, 32) + "\",\"size\":" + std::to_string(b.size) +
                     ",\"encoding\":\"identity\",\"engine\":\"demodel_b200\",\"abi\":" + std::to_string(DM_ABI_VERSION) +
                     ",\"headers\":{";
@@ -538,6 +539,8 @@ std::shared_ptr<Blob> publish(dm_engine *e, const Digest &d, uint64_t size, std:
             lru_touch(e, b.get());
         } else if (it != e->blobs.end()) {   // known on disk only: re-home into HBM
             b = it->second;
+            if (b->size != size) b->sidecar.clear();     // an entry dm_cache_promote registered from an unverified file:
+            b->size = size;                              // the verified length wins, and a sidecar stating another goes
             b->extents = kept; kept.clear();
             b->in_hbm = true; lru_touch(e, b.get());
         } else {
@@ -578,6 +581,7 @@ void publish_many(dm_engine *e, const std::vector<Verified> &items)
                 to_free.push_back(v.x);
             } else if (it != e->blobs.end()) {                         // on disk only: re-home
                 Blob *b = it->second.get();
+                b->size = v.size;
                 b->extents.assign(1, v.x);
                 b->in_hbm = true; lru_touch(e, b);
             } else {

@@ -1,6 +1,7 @@
 // engine_internal.hpp - types, constants and internal entry points shared by the engine's translation units:
 //   engine_core.cu    extents, ring slabs, CAS commit / eviction, the pump (launch decisions), the disk tier
-//   engine_api.cu     C-ABI: engine lifecycle, streams (ingest, ranges, checkpoint / resume, zero-copy windows)
+//   engine_api.cu     C-ABI: engine lifecycle, streams (ingest, ranges, checkpoint / resume, zero-copy windows),
+//                     promotion of disk-tier blobs back into HBM (internal streams)
 //   engine_cache.cu   C-ABI: hit serving (readers, followers), device-resident ingest, the synthetic generator
 // Not installed, not part of the boundary (that is include/demodel_b200.h).
 #pragma once
@@ -116,6 +117,7 @@ struct Blob {
     bool on_disk = false;
     bool spill_done = false;
     std::vector<std::pair<std::string, std::string>> meta;   // response headers to replay on a hit
+    std::string sidecar;                  // promoted from the disk tier (dm_cache_promote): its .meta text, replayed as is
 };
 
 struct Slab { uint8_t *host; uint8_t *dev; };   // dev: same slab of the device-side mirror (verify-only streams)
@@ -307,6 +309,7 @@ struct dm_engine {
     std::atomic<bool> ring_starved{false};
     std::mutex slot_mu;              // state / digest slots: a lock of their own, so that opening and closing tiny bodies from
     std::vector<uint32_t> free_slots;                // many threads does not queue on the index lock `mu`
+    size_t promote_reserved = 0;     // slots running dm_cache_promote calls may take (slot_mu)
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp
     std::unordered_map<Digest, std::weak_ptr<Stream>, DigestHash> inflight;   // open streams by expected digest

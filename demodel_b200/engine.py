@@ -232,6 +232,19 @@ class Engine:
         check(rc, "dm_cache_evict")
         return True
 
+    def promote(self, digests: Sequence[bytes]) -> list[int]:
+        """dm_cache_promote: bring cached blobs back into HBM, each disk copy verified on the GPU as it loads.
+        One status per digest: DM_OK (in HBM now), DM_ENOENT, DM_ENOMEM, DM_EIO, DM_ECUDA or DM_ECORRUPT (the disk
+        copy did not hash to its name and was removed)."""
+        digests = list(digests)
+        if any(len(d) != 32 for d in digests):
+            raise ValueError("every digest must be 32 bytes")
+        status = (C.c_int32 * max(len(digests), 1))()
+        blob = b"".join(digests)
+        check(self._lib.dm_cache_promote(self._h, C.cast(C.c_char_p(blob), C.c_void_p) if digests else None,
+                                         len(digests), status), "dm_cache_promote")
+        return list(status[:len(digests)])
+
     # -- URL-keyed requests (the OnRequest hook is handed a URL) -----------------------
     def alias_put(self, key: str, digest: bytes) -> None:
         check(self._lib.dm_cache_alias_put(self._h, key.encode(), _digest_arg(digest)), "dm_cache_alias_put")

@@ -405,6 +405,41 @@ func (p *Pool) Follow(digest *[32]byte) *HitReader {
 	return &HitReader{e: e, id: id, Size: int64(size)} // Size 0 = unknown: send chunked
 }
 
+// Promote brings cached blobs back into HBM (dm_cache_promote): each disk copy is loaded and verified on the GPU
+// that owns its digest, the engines in parallel.  It blocks until every blob has a status: 0 (DM_OK, in HBM now)
+// or a negative dm_err - DM_ENOENT, DM_ENOMEM, DM_EIO, DM_ECUDA, or DM_ECORRUPT when the disk copy did not hash to
+// its name and was removed.  Run it in a goroutine after start-up; hits are served from disk meanwhile.
+func (p *Pool) Promote(digests [][32]byte) ([]int, error) {
+	status := make([]int, len(digests))
+	byEngine := make(map[*C.dm_engine][]int)
+	for i := range digests {
+		e := p.engineFor(&digests[i])
+		byEngine[e] = append(byEngine[e], i)
+	}
+	errs := make(chan error, len(byEngine))
+	for e, idx := range byEngine {
+		go func(e *C.dm_engine, idx []int) {
+			buf := make([][32]byte, len(idx))
+			for k, i := range idx {
+				buf[k] = digests[i]
+			}
+			st := make([]C.int32_t, len(idx))
+			err := check(e, 0, C.dm_cache_promote(e, (*C.uint8_t)(unsafe.Pointer(&buf[0][0])), C.uint32_t(len(idx)), &st[0]))
+			for k, i := range idx {
+				status[i] = int(st[k])
+			}
+			errs <- err
+		}(e, idx)
+	}
+	var first error
+	for range byEngine {
+		if err := <-errs; err != nil && first == nil {
+			first = err
+		}
+	}
+	return status, first
+}
+
 // ---- requests are URLs, not digests (start.go:197-200) ------------------------------------------------------
 
 // SetURL records the request URL with the body: it goes into the sidecar, and once the body has verified the

@@ -48,7 +48,8 @@ typedef enum dm_err {
     DM_ESTATE    = -5,   /* call not valid in the stream's current state */
     DM_EIO       = -6,   /* on-disk CAS tier I/O error */
     DM_ENODEV    = -7,   /* no CUDA device / device ordinal out of range */
-    DM_ERANGE    = -8    /* offset beyond blob end */
+    DM_ERANGE    = -8,   /* offset beyond blob end */
+    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote) */
 } dm_err;
 
 typedef struct dm_engine dm_engine;   /* opaque; owned by caller between create/destroy */
@@ -227,6 +228,31 @@ int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t
 int dm_cache_meta(dm_engine *e, uint64_t reader, char *buf, size_t cap, size_t *len);
 int dm_cache_close(dm_engine *e, uint64_t reader);
 int dm_cache_evict(dm_engine *e, const uint8_t digest[32]);   /* HBM tier only; disk copy stays */
+/* Bring cached blobs back into HBM, verifying each disk copy on the GPU as it loads.  A blob leaves HBM when it is
+ * evicted or the engine restarts, and dm_cache_open serves it from <cas_dir>/blobs/ from then on, unverified and
+ * without dm_cache_device_extents.  This reads each file into the pinned ring, DMAs it into a fresh HBM extent and
+ * hashes it there as an ordinary stream with the digest as its expected value; many files load at once, so their
+ * hash chains share launches.  Blocks until every status is known.  status_out[i]:
+ *   DM_OK        it was in HBM when the call looked, or its disk copy was loaded and hashed to digests[i].  HBM is
+ *                an LRU cache: a call over more bytes than hbm_cas_bytes evicts blobs it promoted earlier to make
+ *                room for later ones (they stay DM_OK, and stay on disk), as any other ingest may evict them later
+ *   DM_ENOENT    on neither tier
+ *   DM_ENOMEM    larger than hbm_cas_bytes, no room even after LRU eviction, or no stream slot to spare (see
+ *                below): left on disk, untouched
+ *   DM_EIO       the file could not be read: left untouched
+ *   DM_ECUDA     a copy or launch failed while it loaded: left untouched, not in HBM
+ *   DM_ECORRUPT  the disk copy does NOT hash to its name (or is shorter / longer than its sidecar says):
+ *                file and sidecar removed, the digest is now a miss
+ * A file is removed only if its path still names the file that was read (one a stream published meanwhile stays).
+ * A disk reader that opened a corrupt file before keeps its descriptor and reads what the file holds.  The file and
+ * sidecar of a verified blob stay as they are (nothing is written back), and dm_cache_meta returns the sidecar's text
+ * unchanged; a blob without a sidecar is promoted with no headers.  Duplicates in digests[] are loaded once.  The
+ * call opens at most half of the stream slots that are free when it starts and not reserved by other running calls,
+ * so it never takes the last one from dm_stream_open; with fewer than two such slots it loads nothing, and each blob
+ * it would have loaded is DM_ENOMEM.
+ * Returns DM_OK once every status is filled; DM_EINVAL on bad arguments; DM_ESTATE on a DM_F_NO_HBM_CAS engine
+ * (there is no HBM tier).  Without cas_dir every blob not already in HBM is DM_ENOENT. */
+int dm_cache_promote(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out);
 /* Request coalescing: the blob is not cached yet but another connection is
  * ingesting it right now (a stream opened with this expected digest).  The
  * reader follows that body out of HBM: dm_cache_read blocks until bytes past
