@@ -111,6 +111,8 @@ SIGNATURES = {
     "dm_cache_close": (C.c_int, [_P, C.c_uint64]),
     "dm_cache_evict": (C.c_int, [_P, _P]),
     "dm_cache_promote": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
+    "dm_cache_verify": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
+    "dm_cache_list": (C.c_int, [_P, _P, _P, _U64P, C.c_uint32, C.POINTER(C.c_uint32)]),
     "dm_cache_follow": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_alias_put": (C.c_int, [_P, C.c_char_p, _P]),
     "dm_cache_alias_get": (C.c_int, [_P, C.c_char_p, _P]),

@@ -160,7 +160,10 @@ void dm_engine_destroy(dm_engine *e)
     for (auto &t : e->disk_threads) if (t.joinable()) t.join();
     for (auto &m : e->streams)                    // disk-backed streams nobody finished: their files go with the engine
         for (auto &kv : m)
-            if (kv.second->fd >= 0) { close(kv.second->fd); unlink(kv.second->path.c_str()); }
+            if (kv.second->fd >= 0) {
+                close(kv.second->fd);
+                if (!kv.second->check_only) unlink(kv.second->path.c_str());     // (a check's file is a blob of the tier)
+            }
     cudaDeviceSynchronize();
     for (auto &m : e->readers) for (auto &kv : m) if (kv.second->fd >= 0) close(kv.second->fd);
     for (Cycle &c : e->cycles) {
@@ -352,7 +355,7 @@ static int engine_create(const dm_config *cfg, dm_engine **out)
         }
     }
     e->pump = std::thread(pump_main, e);
-    if (e->cfg.flags & DM_F_DISK_DIRECT)
+    if (!e->cas_dir.empty())          // disk-backed streams, and dm_cache_verify on any engine with a disk tier
         for (int i = 0; i < kDiskThreads; ++i) e->disk_threads.emplace_back(disk_main, e);
     for (int i = 0; i < kCompleters; ++i) e->completers.emplace_back(completer_main, e);
     if (!e->cas_dir.empty())
@@ -1090,7 +1093,7 @@ static int stream_abort_impl(dm_engine *e, uint64_t id)
             free_now = s->jobs_inflight == 0;
             s->cv.wait(g, [&] { return s->disk_writes == 0 && s->disk_reads == 0 && !s->publishing; });
             if (s->fd >= 0) { close(s->fd); s->fd = -1; }
-            if (!s->path.empty()) unlink(s->path.c_str());
+            if (!s->path.empty() && !s->check_only) unlink(s->path.c_str());
         }
         if (!s->staged.empty()) {            // their DMAs may be in flight: drain before the ring reuses them
             cudaSetDevice(e->device);
@@ -1139,7 +1142,8 @@ struct Promotion {
     std::shared_ptr<Blob> mine;           // the disk-only entry this promotion registered (none if one existed)
 };
 
-// The sidecar's top-level "size" (it precedes "headers", so the first match is it).
+// The sidecar's top-level "size" (it precedes "headers", so the first match is it).  The number must be followed by
+// ',' or '}': a sidecar read while write_sidecar is still writing it may end in the middle of the number.
 bool sidecar_size(const std::string &j, uint64_t *size)
 {
     const size_t p = j.find("\"size\":");
@@ -1147,7 +1151,7 @@ bool sidecar_size(const std::string &j, uint64_t *size)
     const char *s = j.c_str() + p + 7;
     char *end = nullptr;
     *size = strtoull(s, &end, 10);
-    return end != s;
+    return end != s && (*end == ',' || *end == '}');
 }
 
 // The disk copy under the index entry of `d` is bad or unchecked: forget an entry that is not in HBM, and spill
@@ -1191,6 +1195,34 @@ void promote_undo(dm_engine *e, Promotion &p)
     if (p.mine) forget_disk_copy(e, p.d, p.mine.get());
 }
 
+// Open the disk copy of `d` for a check: *fd open O_RDONLY, `seen` its fstat, `side` its sidecar text ("" if none).
+// DM_ENOENT without a file (or a cas_dir), DM_EIO when it cannot be opened, DM_ECORRUPT (file and sidecar dropped)
+// when its size is not the one its sidecar states.
+int open_disk_copy(dm_engine *e, const Digest &d, int *fd, struct stat *seen, std::string *side)
+{
+    *fd = -1;
+    if (e->cas_dir.empty()) return DM_ENOENT;
+    const std::string path = blob_path(e, d.b);
+    const int f = open(path.c_str(), O_RDONLY | O_CLOEXEC);
+    if (f < 0) return errno == ENOENT ? DM_ENOENT : fail(DM_EIO, "could not open the disk tier file");
+    if (fstat(f, seen) != 0) { close(f); return fail(DM_EIO, "could not stat the disk tier file"); }
+    side->clear();
+    if (FILE *mf = fopen((path + ".meta").c_str(), "r")) {
+        char tmp[4096];
+        size_t k;
+        while ((k = fread(tmp, 1, sizeof tmp, mf)) > 0) side->append(tmp, k);
+        fclose(mf);
+    }
+    uint64_t claimed;
+    if (!side->empty() && sidecar_size(*side, &claimed) && claimed != (uint64_t)seen->st_size) {
+        close(f);
+        drop_corrupt(e, d, *seen);
+        return fail(DM_ECORRUPT, "disk tier file is not the size its sidecar says");
+    }
+    *fd = f;
+    return DM_OK;
+}
+
 // Start loading one blob.  Returns 1 with p.stream open (and flushed unless p.tiny), or the blob's final status.
 // `tiny_buf` holds tiny_max bytes: a tiny body is read there and written into its stream's private buffer, so that it
 // holds no ring slab while it waits for its batch's flush.  `may_open`: false when the call has no stream slot to spare.
@@ -1201,25 +1233,10 @@ int promote_start(dm_engine *e, Promotion &p, uint8_t *tiny_buf, bool may_open)
         auto it = e->blobs.find(p.d);
         if (it != e->blobs.end() && it->second->in_hbm) return DM_OK;
     }
-    if (e->cas_dir.empty()) return DM_ENOENT;
-    const std::string path = blob_path(e, p.d.b);
-    const int fd = open(path.c_str(), O_RDONLY | O_CLOEXEC);
-    if (fd < 0) return errno == ENOENT ? DM_ENOENT : fail(DM_EIO, "could not open the disk tier file");
-    if (fstat(fd, &p.seen) != 0) { close(fd); return fail(DM_EIO, "could not stat the disk tier file"); }
-    const uint64_t size = (uint64_t)p.seen.st_size;
+    int fd;
     std::string side;
-    if (FILE *mf = fopen((path + ".meta").c_str(), "r")) {
-        char tmp[4096];
-        size_t k;
-        while ((k = fread(tmp, 1, sizeof tmp, mf)) > 0) side.append(tmp, k);
-        fclose(mf);
-    }
-    uint64_t claimed;
-    if (!side.empty() && sidecar_size(side, &claimed) && claimed != size) {
-        close(fd);
-        drop_corrupt(e, p.d, p.seen);
-        return fail(DM_ECORRUPT, "disk tier file is not the size its sidecar says");
-    }
+    if (int rc = open_disk_copy(e, p.d, &fd, &p.seen, &side); rc != DM_OK) return rc;
+    const uint64_t size = (uint64_t)p.seen.st_size;
     // checked here: a stream with this size_hint would silently become verify-only or disk-backed
     if (size > e->cfg.hbm_cas_bytes) { close(fd); return fail(DM_ENOMEM, "blob is larger than the HBM arena"); }
     if (!may_open) { close(fd); return fail(DM_ENOMEM, "no stream slot to spare for a promotion"); }
@@ -1350,10 +1367,246 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
     return DM_OK;
 }
 
+// ---- checks of disk-tier files in place (dm_cache_verify) -------------------------------------------------------
+// A stored file is a disk-backed stream whose every byte is already written.  Each check is an internal stream opened
+// with expect = the digest: its fd is the blob file, [0, size) counts as written, and it is finished at once, so the
+// disk threads read the file back into ring slabs (at most two per check on the hash side) and the pump hashes them
+// as verify-only jobs.  Files of at most tiny_max bytes are read here instead and travel in packs as hash-only members,
+// many to a launch.  No check holds an arena extent, and a verdict is all a check produces.
+
+namespace {
+
+constexpr int kVerifyThreads = 4;         // threads that open checks and collect their verdicts
+constexpr size_t kVerifyTinyBatch = 256;  // tiny checks flushed together: they share pack DMAs and launches
+
+struct Check {
+    Digest d;
+    int32_t status = DM_ENOENT;
+    uint64_t stream = 0;                  // open: the verdict is still to be collected
+    bool tiny = false;                    // in its stream's private buffer until flushed, then in a pack
+    struct stat seen{};                   // the file that was read (st_dev / st_ino)
+};
+
+bool blob_in_hbm(dm_engine *e, const Digest &d)
+{
+    std::lock_guard<std::mutex> g(e->mu);
+    auto it = e->blobs.find(d);
+    return it != e->blobs.end() && it->second->in_hbm;
+}
+
+// Open the check of the file `fd` (c.seen is its fstat).  The stream takes over fd, or it is closed here.  Returns 1
+// with c.stream open (a disk-backed check already finishing, a tiny one waiting for its flush) or c's final status.
+int check_open(dm_engine *e, Check &c, int fd)
+{
+    const uint64_t size = (uint64_t)c.seen.st_size;
+    auto sp = std::make_shared<Stream>();
+    sp->has_expect = true;
+    sp->expect = c.d;
+    sp->check_only = sp->verify_only = true;
+    sp->size_hint = size;
+    c.tiny = e->tiny_max && size <= e->tiny_max;
+    if (c.tiny) {
+        sp->small.reset(new uint8_t[std::max<uint64_t>(size, 1)]);
+        sp->small_cap = (uint32_t)size;
+        uint64_t off = 0;
+        while (off < size) {
+            const ssize_t got = pread(fd, sp->small.get() + off, size - off, (off_t)off);
+            if (got < 0 && errno == EINTR) continue;
+            if (got <= 0) break;                         // a read error, or the file shrank since fstat
+            off += (uint64_t)got;
+        }
+        close(fd);
+        if (off < size) return fail(DM_EIO, "could not read the disk tier file");
+        sp->small_fill = (uint32_t)size;
+        sp->received = size;
+    } else {
+        sp->disk = true;
+        sp->fd = fd;
+        sp->path = blob_path(e, c.d.b);
+        if (size) add_interval(sp->written, 0, size);
+        sp->dma_issued = sp->landed = sp->received = size;
+    }
+    {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        if (e->free_slots.empty()) {
+            if (sp->fd >= 0) close(sp->fd);
+            return fail(DM_ENOMEM, "max_streams reached");
+        }
+        sp->slot = e->free_slots.back();
+        e->free_slots.pop_back();
+    }
+    sp->id = e->next_id.fetch_add(1);
+    {
+        const int k = (int)(sp->id % kStripes);
+        std::lock_guard<std::mutex> g(e->stripe_mu[k]);
+        e->streams[k][sp->id] = sp;
+        e->n_streams++;
+    }
+    if (!c.tiny) {                                       // flushed straight away: every byte is already in the file
+        std::lock_guard<std::mutex> g(sp->mu);
+        sp->st = St::Finishing;
+        disk_feed(e, sp);
+        mark_dirty(e, sp, nullptr);
+    }
+    c.stream = sp->id;
+    return 1;
+}
+
+int check_verdict(dm_engine *e, Check &c)
+{
+    uint8_t got[32];
+    int matched = 0;
+    const int rc = stream_finish_impl(e, c.stream, got, &matched);
+    if (rc != DM_OK) {                                   // a failed read, copy or launch: the file is left untouched
+        stream_abort_impl(e, c.stream);                  // (an id finish released just says so)
+        return rc;
+    }
+    if (matched) return DM_OK;
+    drop_corrupt(e, c.d, c.seen);
+    return DM_ECORRUPT;
+}
+
+// A directory entry of blobs/sha256/<aa>/ that names a blob: 64 lowercase hex digits starting with <aa>.
+bool blob_name(const char *name, const char aa[2], Digest *d)
+{
+    return strlen(name) == 64 && name[0] == aa[0] && name[1] == aa[1] && digest_from_hex(name, d->b) &&
+           hex_of(d->b, 32) == name;
+}
+
+}  // namespace
+
+static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
+{
+    if (!e || (n && (!digests || !status_out))) return fail(DM_EINVAL, "null argument");
+    std::vector<Check> work;
+    std::vector<uint32_t> slot_of(n);
+    {
+        std::unordered_map<Digest, uint32_t, DigestHash> first;
+        for (uint32_t i = 0; i < n; ++i) {
+            Digest d;
+            memcpy(d.b, digests + 32ull * i, 32);
+            auto ins = first.emplace(d, (uint32_t)work.size());
+            if (ins.second) { work.emplace_back(); work.back().d = d; }
+            slot_of[i] = ins.first->second;
+        }
+    }
+    // read-backs (and a tiny check that finds no pack) stage slabs in the ring's device mirror
+    const bool ring_ok = e->cas_dir.empty() || work.empty() || ensure_dev_ring(e) == DM_OK;
+    // The same slot budget as dm_cache_promote, from the same reservation.  The live proxy keeps its ring: at most a
+    // quarter of the slabs' worth of disk-backed checks are open at once, and each holds at most two slabs.
+    size_t budget;
+    {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        const size_t free = e->free_slots.size();
+        budget = free > e->promote_reserved ? (free - e->promote_reserved) / 2 : 0;
+        e->promote_reserved += budget;
+    }
+    const size_t ring_share = std::max<size_t>(1, e->slab_store.size() / 4);
+    const size_t nthreads = std::min<size_t>({(size_t)kVerifyThreads, work.size(), std::max<size_t>(budget, 1), ring_share});
+    const size_t per_thread = std::max<size_t>(1, budget / std::max<size_t>(nthreads, 1));
+    const size_t disk_per_thread = std::max<size_t>(1, ring_share / std::max<size_t>(nthreads, 1));
+    std::atomic<size_t> next{0};
+    auto checker = [&] {
+        cudaSetDevice(e->device);
+        std::deque<Check *> open;                        // verdict not collected yet (oldest first)
+        std::vector<Check *> unflushed;                  // tiny ones among them, flushed together
+        size_t open_disk = 0;
+        // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
+        auto flush = [&] { for (Check *c : unflushed) stream_flush_impl(e, c->stream); unflushed.clear(); };
+        auto collect = [&] {
+            flush();
+            Check *c = open.front();
+            open.pop_front();
+            if (!c->tiny) --open_disk;
+            c->status = check_verdict(e, *c);
+        };
+        std::string side;
+        for (size_t k; (k = next.fetch_add(1)) < work.size();) {
+            Check &c = work[k];
+            int fd = -1;
+            const int rc = open_disk_copy(e, c.d, &fd, &c.seen, &side);
+            if (rc == DM_ENOENT) { c.status = blob_in_hbm(e, c.d) ? DM_OK : DM_ENOENT; continue; }   // (verified at ingest)
+            if (rc != DM_OK) { c.status = rc; continue; }
+            if (budget == 0 || !ring_ok) {
+                close(fd);
+                c.status = !ring_ok ? fail(DM_ECUDA, "could not allocate the ring's device mirror")
+                                    : fail(DM_ENOMEM, "no stream slot to spare for a check");
+                continue;
+            }
+            const bool tiny = e->tiny_max && (uint64_t)c.seen.st_size <= e->tiny_max;
+            while (!open.empty() && (open.size() >= per_thread || (!tiny && open_disk >= disk_per_thread))) collect();
+            const int st = check_open(e, c, fd);
+            if (st != 1) { c.status = st; continue; }
+            open.push_back(&c);
+            if (c.tiny) unflushed.push_back(&c);
+            else ++open_disk;
+            if (unflushed.size() >= kVerifyTinyBatch) flush();
+        }
+        flush();
+        while (!open.empty()) collect();
+    };
+    std::vector<std::thread> th;
+    for (size_t t = 1; t < nthreads; ++t) th.emplace_back(checker);
+    if (nthreads) checker();
+    for (auto &t : th) t.join();
+    { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved -= budget; }
+    for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
+    return DM_OK;
+}
+
+// ---- listing the disk tier (dm_cache_list) ----------------------------------------------------------------------
+// Stateless: a page starts strictly after the last digest of the one before, so blobs may come and go between calls.
+// Only the prefix directories from after[0] on are read, one at a time, each sorted on its own.
+static int cache_list_impl(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, uint64_t *sizes_out,
+                           uint32_t cap, uint32_t *n_out)
+{
+    if (!e || !n_out || (cap && !digests_out)) return fail(DM_EINVAL, "null argument");
+    *n_out = 0;
+    if (e->cas_dir.empty()) return DM_OK;
+    const std::string root = e->cas_dir + "/blobs/sha256/";
+    uint32_t got = 0;
+    std::vector<Digest> names;
+    for (int p = after ? after[0] : 0; p < 256 && got < cap; ++p) {
+        char aa[3];
+        snprintf(aa, sizeof aa, "%02x", p);
+        const std::string dir = root + aa + "/";
+        DIR *d = opendir(dir.c_str());
+        if (!d) continue;
+        names.clear();
+        while (struct dirent *de = readdir(d)) {
+            Digest dg;
+            if (!blob_name(de->d_name, aa, &dg)) continue;                  // .meta, .part and strays
+            if (after && memcmp(dg.b, after, 32) <= 0) continue;
+            names.push_back(dg);
+        }
+        closedir(d);
+        std::sort(names.begin(), names.end(), [](const Digest &a, const Digest &b) { return memcmp(a.b, b.b, 32) < 0; });
+        for (const Digest &dg : names) {
+            if (got == cap) break;
+            struct stat st;
+            if (stat((dir + hex_of(dg.b, 32)).c_str(), &st) != 0 || !S_ISREG(st.st_mode)) continue;   // gone meanwhile
+            memcpy(digests_out + 32ull * got, dg.b, 32);
+            if (sizes_out) sizes_out[got] = (uint64_t)st.st_size;
+            ++got;
+        }
+    }
+    *n_out = got;
+    return DM_OK;
+}
+
 // ---- exported wrappers: file the error text under the stream id (dm_error_detail) ----
 int dm_cache_promote(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
 {
     return note_err(e, 0, cache_promote_impl(e, digests, n, status_out));
+}
+int dm_cache_verify(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
+{
+    return note_err(e, 0, cache_verify_impl(e, digests, n, status_out));
+}
+int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, uint64_t *sizes_out, uint32_t cap,
+                  uint32_t *n_out)
+{
+    return note_err(e, 0, cache_list_impl(e, after, digests_out, sizes_out, cap, n_out));
 }
 int dm_stream_suspend(dm_engine *e, uint64_t id, uint64_t *resume_from) { return note_err(e, id, stream_suspend_impl(e, id, resume_from)); }
 int dm_stream_resume_saved(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, uint64_t *resume_from)

@@ -342,7 +342,7 @@ int submit_slab(dm_engine *e, const std::shared_ptr<Stream> &sp)
     const uint32_t n = s->cur_fill;
     s->cur = nullptr; s->cur_fill = 0;
     if (n == 0) { slab_put(e, slab); return DM_OK; }
-    e->st_ingested.fetch_add(n, std::memory_order_relaxed);       // per slab, not per write: one shared line, many writer threads
+    if (!s->check_only) e->st_ingested.fetch_add(n, std::memory_order_relaxed);   // per slab, not per write: one shared line, many writer threads
     if (s->disk) {
         disk_write(e, sp, slab, s->dma_issued, n);
         s->dma_issued += n;
@@ -419,12 +419,14 @@ bool pack_tiny_body(dm_engine *e, Stream *s)
 {
     const uint32_t n = s->cur ? s->cur_fill : s->small_fill;
     const uint8_t *from = s->cur ? s->cur->host : s->small.get();
-    if (!from || n == 0 || n > e->tiny_max || s->verify_only || s->dma_issued || s->resume_base || s->carry_fill ||
-        !s->parts.empty() || !s->islands.empty() || e->pack_dev_base == nullptr)
+    if (!from || n == 0 || n > e->tiny_max || (s->verify_only && !s->check_only) || s->dma_issued || s->resume_base ||
+        s->carry_fill || !s->parts.empty() || !s->islands.empty() || e->pack_dev_base == nullptr)
         return false;
-    if (ensure_capacity(e, s, n) != DM_OK) return false;              // (the ordinary path reports the ENOMEM)
-    uint64_t contig = 0;
-    if (!seg_at(e, s->extents, 0, &contig) || contig < n) return false;
+    if (!s->check_only) {                      // a check is a hash-only member: no extent, its job's dst stays null
+        if (ensure_capacity(e, s, n) != DM_OK) return false;          // (the ordinary path reports the ENOMEM)
+        uint64_t contig = 0;
+        if (!seg_at(e, s->extents, 0, &contig) || contig < n) return false;
+    }
     const uint32_t need = (uint32_t)round_up(n, kAlign);
     std::shared_ptr<Pack> pk;
     uint32_t off;
@@ -449,12 +451,13 @@ bool pack_tiny_body(dm_engine *e, Stream *s)
         off = pk->fill;
         memcpy(pk->slab->host + off, from, n);
         pk->fill += need;
+        pk->bytes += n;
         pk->refs.fetch_add(1);
     }
     s->pack = pk; s->pack_off = off; s->pack_len = n;
     if (s->cur) { slab_put(e, s->cur); s->cur = nullptr; s->cur_fill = 0; }     // the body's own slab is free again at once
     s->small.reset(); s->small_fill = 0; s->small_cap = 0;
-    e->st_ingested.fetch_add(n, std::memory_order_relaxed);
+    if (!s->check_only) e->st_ingested.fetch_add(n, std::memory_order_relaxed);
     e->st_packed++;
     return true;
 }
@@ -681,7 +684,7 @@ void complete_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, const uint
     g.unlock();
     std::shared_ptr<Blob> b;
     if (matched && whole && !s->verify_only) b = publish(e, d, size, ext, &meta);
-    else { free_extents(e, ext); if (!matched) e->st_mismatch++; }
+    else { free_extents(e, ext); if (!matched && !s->check_only) e->st_mismatch++; }
     g.lock();
     s->blob = b;
     s->st = St::Done;
@@ -1036,7 +1039,7 @@ void pump_main(dm_engine *e)
         for (auto &pk : sealed) {
             const cudaError_t err = cudaMemcpyAsync(pk->dev, pk->slab->host, pk->fill, cudaMemcpyHostToDevice, e->copy_stream[0]);
             if (err != cudaSuccess) { (void)cudaGetLastError(); pk->failed.store(true); }
-            else e->st_h2d += pk->fill;
+            else e->st_h2d += pk->bytes;
             e->slabs_returning.fetch_add(1, std::memory_order_relaxed);
             slabs.push_back(SentSlab{pk->slab, nullptr, 0});     // back to the ring with the next copy-event batch (step 4)
             pk->slab = nullptr;
@@ -1211,7 +1214,7 @@ int ensure_dev_ring(dm_engine *e)
     return DM_OK;
 }
 
-// ---- disk-backed streams (DM_F_DISK_DIRECT) ------------------------------------------
+// ---- disk-backed streams (DM_F_DISK_DIRECT) and checks of disk-tier files (dm_cache_verify) ---------------
 // The client writes into ring slabs as on every stream; a full slab (or a recalled partial one, or a range part)
 // is pwritten at its blob offset by a disk thread and returns to the ring when the write completes, so the
 // client runs at the speed of the network and the disk.  The hash follows from the file: a disk thread reads
@@ -1347,6 +1350,14 @@ static void disk_task_publish(dm_engine *e, DiskTask &t)
 {
     Stream *s = t.sp.get();
     std::unique_lock<std::mutex> g(s->mu);
+    if (s->check_only) {                        // dm_cache_verify: the verdict is all; the file is the caller's to judge
+        if (s->fd >= 0) { close(s->fd); s->fd = -1; }
+        s->publishing = false;
+        if (s->st != St::Aborted) s->st = St::Done;
+        g.unlock();
+        s->cv.notify_all();
+        return;
+    }
     const bool whole = s->resume_base == 0 ||
                        (s->prefix_cover.size() == 1 && s->prefix_cover.begin()->first == 0 &&
                         s->prefix_cover.begin()->second >= s->resume_base);

@@ -1,7 +1,8 @@
 // engine_internal.hpp - types, constants and internal entry points shared by the engine's translation units:
 //   engine_core.cu    extents, ring slabs, CAS commit / eviction, the pump (launch decisions), the disk tier
 //   engine_api.cu     C-ABI: engine lifecycle, streams (ingest, ranges, checkpoint / resume, zero-copy windows),
-//                     promotion of disk-tier blobs back into HBM (internal streams)
+//                     promotion of disk-tier blobs back into HBM and checks of disk-tier files (internal streams),
+//                     the listing of the disk tier
 //   engine_cache.cu   C-ABI: hit serving (readers, followers), device-resident ingest, the synthetic generator
 // Not installed, not part of the boundary (that is include/demodel_b200.h).
 #pragma once
@@ -71,7 +72,7 @@ constexpr int kIngestMaxChunks = 8;
 constexpr uint32_t kIngestChunkMin = 16384;  // jobs per chunk at least: 512 warps of the lane-per-stream kernel
 constexpr int kCompleters = 2;             // threads that compare / publish finished bodies, so the pump only launches and reaps
 constexpr int kBounceReserve = 2 * kSpillThreads + 2;          // never lent to windows: the spill thread and one-shot reads need some
-constexpr int kDiskThreads = 4;            // DM_F_DISK_DIRECT: file writes, read-backs and publications of disk-backed streams
+constexpr int kDiskThreads = 4;            // file writes, read-backs and publications of disk-backed streams and checks
 
 inline uint64_t round_up(uint64_t x, uint64_t a) { return (x + a - 1) / a * a; }
 
@@ -132,6 +133,7 @@ struct Pack {
     Slab *slab = nullptr;            // host side, handed to the ordinary slab-return path once the DMA is enqueued
     uint8_t *dev = nullptr;          // device staging buffer, back to the pool when the last member's job is reaped
     uint32_t fill = 0;               // bytes used; members sit at 256-byte aligned offsets
+    uint32_t bytes = 0;              // the members' own bytes (h2d_bytes counts these, not the alignment padding)
     std::atomic<uint32_t> refs{0};   // members whose job has not been reaped (or that have not been aborted)
     std::atomic<bool> dma_issued{false};
     std::atomic<bool> failed{false};
@@ -190,6 +192,10 @@ struct Stream {
     uint32_t disk_writes = 0, disk_reads = 0;    // in flight on the disk threads (at most one read)
     bool publishing = false;                     // the final rename / sidecar is running on a disk thread
     bool suspending = false;                     // dm_stream_suspend: no further read-back or launch
+    // dm_cache_verify: a check of a stored file, never a download.  A disk-backed check reads the blob file itself
+    // (fd / path, every byte already written); a tiny one travels in a pack as a hash-only member.  It holds no arena
+    // extent, and its verdict is all it produces: nothing is published, renamed, truncated or unlinked.
+    bool check_only = false;
     // A body announced (Content-Length) as at most tiny_max bytes never takes a ring slab: its bytes gather in this
     // private buffer and go straight into a pack when it finishes.  Anything that needs a real slab (more bytes than
     // announced, range parts, zero-copy windows, checkpoints) moves them into one first (take_slab).
@@ -309,7 +315,7 @@ struct dm_engine {
     std::atomic<bool> ring_starved{false};
     std::mutex slot_mu;              // state / digest slots: a lock of their own, so that opening and closing tiny bodies from
     std::vector<uint32_t> free_slots;                // many threads does not queue on the index lock `mu`
-    size_t promote_reserved = 0;     // slots running dm_cache_promote calls may take (slot_mu)
+    size_t promote_reserved = 0;     // slots running dm_cache_promote / dm_cache_verify calls may take (slot_mu)
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp
     std::unordered_map<Digest, std::weak_ptr<Stream>, DigestHash> inflight;   // open streams by expected digest
@@ -352,7 +358,7 @@ struct dm_engine {
     std::deque<std::shared_ptr<Blob>> spill_q;
     std::vector<std::thread> spillers;   // kSpillThreads writers of the disk tier
 
-    std::mutex disk_mu;                  // DM_F_DISK_DIRECT: the disk threads' queue (taken after a stream mutex, never before)
+    std::mutex disk_mu;                  // disk threads (any engine with a cas_dir): their queue (taken after a stream mutex, never before)
     std::condition_variable disk_cv;
     std::deque<DiskTask> disk_q;
     std::vector<std::weak_ptr<Stream>> disk_starved;   // read-backs that found the ring empty: retried by the disk threads

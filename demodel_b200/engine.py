@@ -245,6 +245,31 @@ class Engine:
                                          len(digests), status), "dm_cache_promote")
         return list(status[:len(digests)])
 
+    def verify(self, digests: Sequence[bytes]) -> list[int]:
+        """dm_cache_verify: hash each disk-tier copy in place on the GPU, without loading it into HBM.  One status per
+        digest: DM_OK, DM_ENOENT, DM_ECORRUPT (the file did not hash to its name, or did not have its sidecar's
+        size, and was removed), DM_EIO, DM_ECUDA or DM_ENOMEM (no stream slot to spare)."""
+        digests = list(digests)
+        if any(len(d) != 32 for d in digests):
+            raise ValueError("every digest must be 32 bytes")
+        status = (C.c_int32 * max(len(digests), 1))()
+        blob = b"".join(digests)
+        check(self._lib.dm_cache_verify(self._h, C.cast(C.c_char_p(blob), C.c_void_p) if digests else None,
+                                        len(digests), status), "dm_cache_verify")
+        return list(status[:len(digests)])
+
+    def list(self, after: Optional[bytes] = None, cap: int = 4096) -> list[tuple[bytes, int]]:
+        """dm_cache_list: up to `cap` (digest, size) pairs of the disk tier in ascending digest order, strictly after
+        `after`.  Fewer than `cap` means the listing is complete; page by passing the last digest returned."""
+        if cap < 0:
+            raise ValueError("cap must be >= 0")
+        digs = (C.c_uint8 * (32 * max(cap, 1)))()
+        sizes = (C.c_uint64 * max(cap, 1))()
+        n = C.c_uint32()
+        check(self._lib.dm_cache_list(self._h, _digest_arg(after), digs, sizes, cap, C.byref(n)), "dm_cache_list")
+        raw = bytes(digs)
+        return [(raw[32 * i:32 * i + 32], sizes[i]) for i in range(n.value)]
+
     # -- URL-keyed requests (the OnRequest hook is handed a URL) -----------------------
     def alias_put(self, key: str, digest: bytes) -> None:
         check(self._lib.dm_cache_alias_put(self._h, key.encode(), _digest_arg(digest)), "dm_cache_alias_put")

@@ -21,9 +21,11 @@ package b200
 import "C"
 
 import (
+	"bytes"
 	"errors"
 	"fmt"
 	"io"
+	"sort"
 	"unsafe"
 )
 
@@ -438,6 +440,81 @@ func (p *Pool) Promote(digests [][32]byte) ([]int, error) {
 		}
 	}
 	return status, first
+}
+
+// Verify checks disk-tier copies in place (dm_cache_verify): each file is hashed on the GPU that owns its digest,
+// the engines in parallel, without loading anything into HBM or evicting anything there.  It blocks until every blob
+// has a status: 0 (DM_OK) or a negative dm_err - DM_ENOENT, DM_EIO, DM_ECUDA, DM_ENOMEM (no stream slot to spare),
+// or DM_ECORRUPT when the file did not hash to its name and was removed.  For a background scrub of the whole tier,
+// page through List and pass each page to Verify.
+func (p *Pool) Verify(digests [][32]byte) ([]int, error) {
+	status := make([]int, len(digests))
+	byEngine := make(map[*C.dm_engine][]int)
+	for i := range digests {
+		e := p.engineFor(&digests[i])
+		byEngine[e] = append(byEngine[e], i)
+	}
+	errs := make(chan error, len(byEngine))
+	for e, idx := range byEngine {
+		go func(e *C.dm_engine, idx []int) {
+			buf := make([][32]byte, len(idx))
+			for k, i := range idx {
+				buf[k] = digests[i]
+			}
+			st := make([]C.int32_t, len(idx))
+			err := check(e, 0, C.dm_cache_verify(e, (*C.uint8_t)(unsafe.Pointer(&buf[0][0])), C.uint32_t(len(idx)), &st[0]))
+			for k, i := range idx {
+				status[i] = int(st[k])
+			}
+			errs <- err
+		}(e, idx)
+	}
+	var first error
+	for range byEngine {
+		if err := <-errs; err != nil && first == nil {
+			first = err
+		}
+	}
+	return status, first
+}
+
+// List returns up to limit blobs of the disk tier of every engine (dm_cache_list), merged in ascending digest order,
+// strictly after `after` (nil: from the start), with their sizes.  Fewer than limit entries means the listing is
+// complete; the next page starts after the last digest returned.
+func (p *Pool) List(after *[32]byte, limit int) ([][32]byte, []uint64, error) {
+	if limit <= 0 {
+		return nil, nil, nil
+	}
+	var from *C.uint8_t
+	if after != nil {
+		from = (*C.uint8_t)(unsafe.Pointer(&after[0]))
+	}
+	type entry struct {
+		d    [32]byte
+		size uint64
+	}
+	var all []entry
+	for _, e := range p.engines {
+		digs := make([][32]byte, limit)
+		sizes := make([]C.uint64_t, limit)
+		var n C.uint32_t
+		if err := check(e, 0, C.dm_cache_list(e, from, (*C.uint8_t)(unsafe.Pointer(&digs[0][0])), &sizes[0], C.uint32_t(limit), &n)); err != nil {
+			return nil, nil, err
+		}
+		for k := 0; k < int(n); k++ {
+			all = append(all, entry{digs[k], uint64(sizes[k])})
+		}
+	}
+	sort.Slice(all, func(a, b int) bool { return bytes.Compare(all[a].d[:], all[b].d[:]) < 0 })
+	if len(all) > limit {
+		all = all[:limit]
+	}
+	digests := make([][32]byte, len(all))
+	sizes := make([]uint64, len(all))
+	for k, x := range all {
+		digests[k], sizes[k] = x.d, x.size
+	}
+	return digests, sizes, nil
 }
 
 // ---- requests are URLs, not digests (start.go:197-200) ------------------------------------------------------

@@ -49,7 +49,7 @@ typedef enum dm_err {
     DM_EIO       = -6,   /* on-disk CAS tier I/O error */
     DM_ENODEV    = -7,   /* no CUDA device / device ordinal out of range */
     DM_ERANGE    = -8,   /* offset beyond blob end */
-    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote) */
+    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote, dm_cache_verify) */
 } dm_err;
 
 typedef struct dm_engine dm_engine;   /* opaque; owned by caller between create/destroy */
@@ -253,6 +253,33 @@ int dm_cache_evict(dm_engine *e, const uint8_t digest[32]);   /* HBM tier only; 
  * Returns DM_OK once every status is filled; DM_EINVAL on bad arguments; DM_ESTATE on a DM_F_NO_HBM_CAS engine
  * (there is no HBM tier).  Without cas_dir every blob not already in HBM is DM_ENOENT. */
 int dm_cache_promote(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out);
+/* Check disk-tier copies in place: hash each file <cas_dir>/blobs/sha256/<aa>/<hex> on the GPU and compare the result
+ * with its name, at any size, with or without an HBM tier (DM_F_NO_HBM_CAS) or DM_F_DISK_DIRECT.  Nothing goes into
+ * the HBM arena: hbm_cas_used, the LRU order and what is cached in HBM stay as they are.  Each file is read back
+ * through the pinned ring by the engine's disk threads, as a disk-backed stream reads its own file; files of at most
+ * 64 KiB share pack DMAs and launches.  Blocks until every status is known.  status_out[i]:
+ *   DM_OK        the file exists, has the size its sidecar states and hashes to digests[i]; or there is no file but
+ *                the blob is in HBM (its spill is pending, or there is no cas_dir): that copy was verified at ingest
+ *   DM_ENOENT    on neither tier
+ *   DM_ECORRUPT  the file does NOT hash to its name, or its size is not its sidecar's "size": file and sidecar removed
+ *                (only if the path still names the file that was read).  A blob that is also in HBM is written to the
+ *                disk tier again from its verified HBM copy; otherwise the digest is now a miss
+ *   DM_EIO       the file could not be opened or read: left untouched
+ *   DM_ECUDA     a copy or launch failed: left untouched
+ *   DM_ENOMEM    no stream slot to spare (the same budget as dm_cache_promote, shared with it): left untouched
+ * A file is checked even when the blob is also in HBM.  Nothing is published, renamed, rewritten or logged;
+ * blobs_committed and blobs_mismatched do not move, bytes_hashed and h2d_bytes grow by the bytes checked.
+ * Duplicates in digests[] are checked once.  At most a quarter of the ring's slabs' worth of files are in flight at
+ * once (each holds at most two slabs), so live streams keep the rest of the ring.
+ * Returns DM_OK once every status is filled; DM_EINVAL on bad arguments. */
+int dm_cache_verify(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out);
+/* Blobs in the disk tier in ascending digest order, strictly after `after` (NULL: from the start).  Up to cap
+ * entries; *n_out < cap means the listing is complete.  sizes_out may be NULL.  Stateless: page by passing the last
+ * digest returned.  Only files named by 64 lowercase hex digits in their own <aa>/ directory are listed (no sidecars,
+ * no partial files); a file removed between the directory read and its stat is skipped.  Without cas_dir: *n_out = 0.
+ * Host code only: "check the whole tier" is dm_cache_list, then dm_cache_verify on each page. */
+int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, uint64_t *sizes_out,
+                  uint32_t cap, uint32_t *n_out);
 /* Request coalescing: the blob is not cached yet but another connection is
  * ingesting it right now (a stream opened with this expected digest).  The
  * reader follows that body out of HBM: dm_cache_read blocks until bytes past
