@@ -23,6 +23,7 @@ DM_ING_HASH_ONLY = 0x1
 DM_ING_REPLACE = 0x2
 DM_ING_FORCE_WIDE = 0x4
 DM_ING_FORCE_DEEP = 0x8
+DM_IMP_LINK = 0x1
 
 
 class DmConfig(C.Structure):
@@ -113,6 +114,8 @@ SIGNATURES = {
     "dm_cache_promote": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_verify": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_list": (C.c_int, [_P, _P, _P, _U64P, C.c_uint32, C.POINTER(C.c_uint32)]),
+    "dm_cache_import": (C.c_int, [_P, C.POINTER(C.c_char_p), _P, C.POINTER(C.c_char_p), C.c_uint32, C.c_uint32, _P,
+                                  C.POINTER(C.c_int32)]),
     "dm_cache_follow": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_alias_put": (C.c_int, [_P, C.c_char_p, _P]),
     "dm_cache_alias_get": (C.c_int, [_P, C.c_char_p, _P]),

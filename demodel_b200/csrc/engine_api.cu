@@ -2,6 +2,7 @@
 #include "engine_internal.hpp"
 
 #include <dirent.h>
+#include <functional>
 #include <sched.h>
 #include <signal.h>
 
@@ -1367,12 +1368,12 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
     return DM_OK;
 }
 
-// ---- checks of disk-tier files in place (dm_cache_verify) -------------------------------------------------------
+// ---- checks of files already written (dm_cache_verify, dm_cache_import) -----------------------------------------
 // A stored file is a disk-backed stream whose every byte is already written.  Each check is an internal stream opened
-// with expect = the digest: its fd is the blob file, [0, size) counts as written, and it is finished at once, so the
-// disk threads read the file back into ring slabs (at most two per check on the hash side) and the pump hashes them
-// as verify-only jobs.  Files of at most tiny_max bytes are read here instead and travel in packs as hash-only members,
-// many to a launch.  No check holds an arena extent, and a verdict is all a check produces.
+// with expect = the digest (when it is known): its fd is the file, [0, size) counts as written, and it is finished at
+// once, so the disk threads read the file back into ring slabs (at most two per check on the hash side) and the pump
+// hashes them as verify-only jobs.  Files of at most tiny_max bytes are read here instead and travel in packs as
+// hash-only members, many to a launch.  No check holds an arena extent, and a verdict is all a check produces.
 
 namespace {
 
@@ -1380,7 +1381,8 @@ constexpr int kVerifyThreads = 4;         // threads that open checks and collec
 constexpr size_t kVerifyTinyBatch = 256;  // tiny checks flushed together: they share pack DMAs and launches
 
 struct Check {
-    Digest d;
+    Digest d;                             // the expected digest (when `known`)
+    bool known = true;
     int32_t status = DM_ENOENT;
     uint64_t stream = 0;                  // open: the verdict is still to be collected
     bool tiny = false;                    // in its stream's private buffer until flushed, then in a pack
@@ -1394,14 +1396,15 @@ bool blob_in_hbm(dm_engine *e, const Digest &d)
     return it != e->blobs.end() && it->second->in_hbm;
 }
 
-// Open the check of the file `fd` (c.seen is its fstat).  The stream takes over fd, or it is closed here.  Returns 1
-// with c.stream open (a disk-backed check already finishing, a tiny one waiting for its flush) or c's final status.
-int check_open(dm_engine *e, Check &c, int fd)
+// Open the check of the file `fd` at `path` (c.seen is its fstat).  The stream takes over fd, or it is closed here.
+// Returns 1 with c.stream open (a disk-backed check already finishing, a tiny one waiting for its flush) or c's final
+// status.
+int check_open(dm_engine *e, Check &c, int fd, const std::string &path)
 {
     const uint64_t size = (uint64_t)c.seen.st_size;
     auto sp = std::make_shared<Stream>();
-    sp->has_expect = true;
-    sp->expect = c.d;
+    sp->has_expect = c.known;
+    if (c.known) sp->expect = c.d;
     sp->check_only = sp->verify_only = true;
     sp->size_hint = size;
     c.tiny = e->tiny_max && size <= e->tiny_max;
@@ -1422,7 +1425,7 @@ int check_open(dm_engine *e, Check &c, int fd)
     } else {
         sp->disk = true;
         sp->fd = fd;
-        sp->path = blob_path(e, c.d.b);
+        sp->path = path;
         if (size) add_interval(sp->written, 0, size);
         sp->dma_issued = sp->landed = sp->received = size;
     }
@@ -1452,19 +1455,108 @@ int check_open(dm_engine *e, Check &c, int fd)
     return 1;
 }
 
+// Collect the verdict of an open check: DM_OK with got[] what the file hashed to, or the error of a failed read, copy
+// or launch (the check is aborted then, its file left untouched).
+int check_finish(dm_engine *e, Check &c, uint8_t got[32], int *matched)
+{
+    const int rc = stream_finish_impl(e, c.stream, got, matched);
+    if (rc != DM_OK) stream_abort_impl(e, c.stream);     // (an id finish released just says so)
+    return rc;
+}
+
 int check_verdict(dm_engine *e, Check &c)
 {
     uint8_t got[32];
     int matched = 0;
-    const int rc = stream_finish_impl(e, c.stream, got, &matched);
-    if (rc != DM_OK) {                                   // a failed read, copy or launch: the file is left untouched
-        stream_abort_impl(e, c.stream);                  // (an id finish released just says so)
-        return rc;
-    }
+    const int rc = check_finish(e, c, got, &matched);
+    if (rc != DM_OK) return rc;
     if (matched) return DM_OK;
     drop_corrupt(e, c.d, c.seen);
     return DM_ECORRUPT;
 }
+
+// What dm_cache_verify and dm_cache_import share: the ring's device mirror (read-backs, and a tiny check that finds
+// no pack, stage slabs there), a slot budget drawn from the reservation dm_cache_promote uses, and kVerifyThreads
+// threads that open checks and collect their verdicts.  The live proxy keeps its ring: at most a quarter of the slabs'
+// worth of disk-backed checks are open at once, and each holds at most two slabs.
+class CheckRun {
+public:
+    CheckRun(dm_engine *e, size_t n_work) : e_(e)
+    {
+        ring_ok_ = e->cas_dir.empty() || n_work == 0 || ensure_dev_ring(e) == DM_OK;
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        const size_t free = e->free_slots.size();
+        budget_ = free > e->promote_reserved ? (free - e->promote_reserved) / 2 : 0;
+        e->promote_reserved += budget_;
+    }
+    ~CheckRun() { std::lock_guard<std::mutex> g(e_->slot_mu); e_->promote_reserved -= budget_; }
+    CheckRun(const CheckRun &) = delete;
+    CheckRun &operator=(const CheckRun &) = delete;
+
+    // DM_OK, or the status of every check this call cannot run
+    int blocked() const
+    {
+        if (!ring_ok_) return fail(DM_ECUDA, "could not allocate the ring's device mirror");
+        if (budget_ == 0) return fail(DM_ENOMEM, "no stream slot to spare for a check");
+        return DM_OK;
+    }
+
+    // prepare(c, &fd, &path): 1 with fd open on the file to check, `path` its name and c.seen its fstat; or c's final
+    // status.  settle(c, rc): c's final status, where rc is 1 when c's check is open and its verdict is due, or the
+    // status with which it could not be opened (fd is closed by then).
+    void run(std::vector<Check> &work, const std::function<int(Check &, int *, std::string *)> &prepare,
+             const std::function<int(Check &, int)> &settle)
+    {
+        dm_engine *e = e_;
+        const size_t ring_share = std::max<size_t>(1, e->slab_store.size() / 4);
+        const size_t nthreads = std::min<size_t>({(size_t)kVerifyThreads, work.size(), std::max<size_t>(budget_, 1), ring_share});
+        const size_t per_thread = std::max<size_t>(1, budget_ / std::max<size_t>(nthreads, 1));
+        const size_t disk_per_thread = std::max<size_t>(1, ring_share / std::max<size_t>(nthreads, 1));
+        std::atomic<size_t> next{0};
+        auto checker = [&] {
+            cudaSetDevice(e->device);
+            std::deque<Check *> open;                        // verdict not collected yet (oldest first)
+            std::vector<Check *> unflushed;                  // tiny ones among them, flushed together
+            size_t open_disk = 0;
+            // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
+            auto flush = [&] { for (Check *c : unflushed) stream_flush_impl(e, c->stream); unflushed.clear(); };
+            auto collect = [&] {
+                flush();
+                Check *c = open.front();
+                open.pop_front();
+                if (!c->tiny) --open_disk;
+                c->status = settle(*c, 1);
+            };
+            std::string path;
+            for (size_t k; (k = next.fetch_add(1)) < work.size();) {
+                Check &c = work[k];
+                int fd = -1;
+                const int rc = prepare(c, &fd, &path);
+                if (rc != 1) { c.status = rc; continue; }
+                if (const int b = blocked()) { close(fd); c.status = settle(c, b); continue; }
+                const bool tiny = e->tiny_max && (uint64_t)c.seen.st_size <= e->tiny_max;
+                while (!open.empty() && (open.size() >= per_thread || (!tiny && open_disk >= disk_per_thread))) collect();
+                const int st = check_open(e, c, fd, path);
+                if (st != 1) { c.status = settle(c, st); continue; }
+                open.push_back(&c);
+                if (c.tiny) unflushed.push_back(&c);
+                else ++open_disk;
+                if (unflushed.size() >= kVerifyTinyBatch) flush();
+            }
+            flush();
+            while (!open.empty()) collect();
+        };
+        std::vector<std::thread> th;
+        for (size_t t = 1; t < nthreads; ++t) th.emplace_back(checker);
+        if (nthreads) checker();
+        for (auto &t : th) t.join();
+    }
+
+private:
+    dm_engine *e_;
+    bool ring_ok_ = true;
+    size_t budget_ = 0;
+};
 
 // A directory entry of blobs/sha256/<aa>/ that names a blob: 64 lowercase hex digits starting with <aa>.
 bool blob_name(const char *name, const char aa[2], Digest *d)
@@ -1490,67 +1582,234 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
             slot_of[i] = ins.first->second;
         }
     }
-    // read-backs (and a tiny check that finds no pack) stage slabs in the ring's device mirror
-    const bool ring_ok = e->cas_dir.empty() || work.empty() || ensure_dev_ring(e) == DM_OK;
-    // The same slot budget as dm_cache_promote, from the same reservation.  The live proxy keeps its ring: at most a
-    // quarter of the slabs' worth of disk-backed checks are open at once, and each holds at most two slabs.
-    size_t budget;
-    {
-        std::lock_guard<std::mutex> g(e->slot_mu);
-        const size_t free = e->free_slots.size();
-        budget = free > e->promote_reserved ? (free - e->promote_reserved) / 2 : 0;
-        e->promote_reserved += budget;
-    }
-    const size_t ring_share = std::max<size_t>(1, e->slab_store.size() / 4);
-    const size_t nthreads = std::min<size_t>({(size_t)kVerifyThreads, work.size(), std::max<size_t>(budget, 1), ring_share});
-    const size_t per_thread = std::max<size_t>(1, budget / std::max<size_t>(nthreads, 1));
-    const size_t disk_per_thread = std::max<size_t>(1, ring_share / std::max<size_t>(nthreads, 1));
-    std::atomic<size_t> next{0};
-    auto checker = [&] {
-        cudaSetDevice(e->device);
-        std::deque<Check *> open;                        // verdict not collected yet (oldest first)
-        std::vector<Check *> unflushed;                  // tiny ones among them, flushed together
-        size_t open_disk = 0;
-        // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
-        auto flush = [&] { for (Check *c : unflushed) stream_flush_impl(e, c->stream); unflushed.clear(); };
-        auto collect = [&] {
-            flush();
-            Check *c = open.front();
-            open.pop_front();
-            if (!c->tiny) --open_disk;
-            c->status = check_verdict(e, *c);
-        };
-        std::string side;
-        for (size_t k; (k = next.fetch_add(1)) < work.size();) {
-            Check &c = work[k];
-            int fd = -1;
-            const int rc = open_disk_copy(e, c.d, &fd, &c.seen, &side);
-            if (rc == DM_ENOENT) { c.status = blob_in_hbm(e, c.d) ? DM_OK : DM_ENOENT; continue; }   // (verified at ingest)
-            if (rc != DM_OK) { c.status = rc; continue; }
-            if (budget == 0 || !ring_ok) {
-                close(fd);
-                c.status = !ring_ok ? fail(DM_ECUDA, "could not allocate the ring's device mirror")
-                                    : fail(DM_ENOMEM, "no stream slot to spare for a check");
-                continue;
-            }
-            const bool tiny = e->tiny_max && (uint64_t)c.seen.st_size <= e->tiny_max;
-            while (!open.empty() && (open.size() >= per_thread || (!tiny && open_disk >= disk_per_thread))) collect();
-            const int st = check_open(e, c, fd);
-            if (st != 1) { c.status = st; continue; }
-            open.push_back(&c);
-            if (c.tiny) unflushed.push_back(&c);
-            else ++open_disk;
-            if (unflushed.size() >= kVerifyTinyBatch) flush();
-        }
-        flush();
-        while (!open.empty()) collect();
-    };
-    std::vector<std::thread> th;
-    for (size_t t = 1; t < nthreads; ++t) th.emplace_back(checker);
-    if (nthreads) checker();
-    for (auto &t : th) t.join();
-    { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved -= budget; }
+    CheckRun run(e, work.size());
+    run.run(work,
+            [&](Check &c, int *fd, std::string *path) -> int {
+                std::string side;
+                const int rc = open_disk_copy(e, c.d, fd, &c.seen, &side);
+                if (rc == DM_ENOENT) return blob_in_hbm(e, c.d) ? DM_OK : DM_ENOENT;     // (verified at ingest)
+                if (rc != DM_OK) return rc;
+                *path = blob_path(e, c.d.b);
+                return 1;
+            },
+            [&](Check &c, int rc) -> int { return rc == 1 ? check_verdict(e, c) : rc; });
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
+    return DM_OK;
+}
+
+// ---- importing files from outside the cache (dm_cache_import) ---------------------------------------------------
+// Each source is first copied (or hard-linked) to a private file under <cas_dir>/incoming/.  That file is checked the
+// way dm_cache_verify checks a tier file and, once it hashes to what was expected, renamed into blobs/ by the thread
+// that collected its verdict: the bytes that get published are the bytes that were hashed, whatever happens to the
+// source meanwhile.  A bad source says nothing about the tier, so nothing here goes through drop_corrupt.
+
+namespace {
+
+struct Import {
+    const char *src = nullptr;
+    std::string staged;                   // the private copy, while it exists
+    uint8_t got[32] = {0};                // what it hashed to (DM_OK, DM_ECORRUPT)
+};
+
+bool on_either_tier(dm_engine *e, const Digest &d)
+{
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        if (e->blobs.find(d) != e->blobs.end()) return true;
+    }
+    struct stat st;
+    return stat(blob_path(e, d.b).c_str(), &st) == 0;
+}
+
+// Copy `src` into a new file `dst`: copy_file_range (a reflink on XFS and btrfs), pread / pwrite where the kernel or
+// the filesystems cannot do that.  Copies up to the end of file as it is now.
+int stage_copy(int src, const std::string &dst)
+{
+    const int out = open(dst.c_str(), O_CREAT | O_TRUNC | O_WRONLY | O_CLOEXEC, 0644);
+    if (out < 0) return fail(DM_EIO, "could not create the staged copy under <cas_dir>/incoming");
+    bool plain = false;
+    std::unique_ptr<uint8_t[]> buf;
+    constexpr size_t kBuf = 1 << 20;
+    loff_t off = 0;
+    int rc = DM_OK;
+    for (;;) {
+        if (!plain) {
+            loff_t in_off = off, out_off = off;
+            const ssize_t r = copy_file_range(src, &in_off, out, &out_off, 1 << 30, 0);
+            if (r > 0) { off += r; continue; }
+            if (r == 0) break;
+            if (errno == EINTR) continue;
+            if (errno != EXDEV && errno != ENOSYS && errno != EINVAL && errno != EOPNOTSUPP) {
+                rc = fail(DM_EIO, "could not copy the file into <cas_dir>/incoming");
+                break;
+            }
+            plain = true;
+            buf.reset(new uint8_t[kBuf]);
+        }
+        const ssize_t r = pread(src, buf.get(), kBuf, off);
+        if (r < 0 && errno == EINTR) continue;
+        if (r < 0) { rc = fail(DM_EIO, "could not read the file to import"); break; }
+        if (r == 0) break;
+        ssize_t w = 0;
+        while (w < r) {
+            const ssize_t k = pwrite(out, buf.get() + w, (size_t)(r - w), off + w);
+            if (k < 0 && errno == EINTR) continue;
+            if (k <= 0) break;
+            w += k;
+        }
+        if (w < r) { rc = fail(DM_EIO, "could not write the staged copy under <cas_dir>/incoming"); break; }
+        off += r;
+    }
+    if (close(out) != 0 && rc == DM_OK) rc = fail(DM_EIO, "could not write the staged copy under <cas_dir>/incoming");
+    return rc;
+}
+
+// Open the source of `im`, stage it and open the staged file for its check (prepare of CheckRun::run).
+int import_prepare(dm_engine *e, const CheckRun &run, uint32_t flags, Check &c, Import &im, int *fd, std::string *path)
+{
+    if (c.known && on_either_tier(e, c.d)) {             // checking the copy that is there is dm_cache_verify's job
+        memcpy(im.got, c.d.b, 32);
+        return DM_OK;
+    }
+    // O_NONBLOCK: opening a FIFO must not wait for a writer (it is refused below like every other non-regular file)
+    const int src = open(im.src, O_RDONLY | O_CLOEXEC | O_NONBLOCK);
+    if (src < 0)
+        return errno == ENOENT || errno == ENOTDIR ? fail(DM_ENOENT, "no such file") : fail(DM_EIO, "could not open the file to import");
+    struct stat st;
+    if (fstat(src, &st) != 0) { close(src); return fail(DM_EIO, "could not stat the file to import"); }
+    if (!S_ISREG(st.st_mode)) { close(src); return fail(DM_EINVAL, "not a regular file"); }
+    if (const int b = run.blocked()) { close(src); return b; }
+    im.staged = incoming_path(e, e->next_id.fetch_add(1));
+    bool linked = false;
+    if (flags & DM_IMP_LINK) {
+        // ENOENT: the source was replaced (renamed over) since it was opened, and the file that is open has no name
+        // left to link: it is copied from the open descriptor like one on another filesystem
+        linked = linkat(AT_FDCWD, im.src, AT_FDCWD, im.staged.c_str(), AT_SYMLINK_FOLLOW) == 0;
+        if (!linked && errno != EXDEV && errno != EPERM && errno != ENOENT) {
+            close(src);
+            im.staged.clear();
+            return fail(DM_EIO, "could not link the file into <cas_dir>/incoming");
+        }
+    }
+    int rc = linked ? DM_OK : stage_copy(src, im.staged);
+    close(src);
+    if (rc == DM_OK) {
+        *fd = open(im.staged.c_str(), O_RDONLY | O_CLOEXEC);
+        if (*fd < 0) rc = fail(DM_EIO, "could not open the staged copy");
+        else if (fstat(*fd, &c.seen) != 0) { close(*fd); rc = fail(DM_EIO, "could not stat the staged copy"); }
+    }
+    if (rc != DM_OK) {
+        unlink(im.staged.c_str());
+        im.staged.clear();
+        return rc;
+    }
+    *path = im.staged;
+    return 1;
+}
+
+// The verdict of an import's check is due: publish the staged file when it hashed to what was expected.
+int import_publish(dm_engine *e, Check &c, Import &im)
+{
+    int matched = 0;
+    const int rc = check_finish(e, c, im.got, &matched);
+    if (rc != DM_OK) { memset(im.got, 0, 32); return rc; }
+    if (!matched) return fail(DM_ECORRUPT, "the file does not hash to the digest it was imported under");
+    if (e->cfg.flags & DM_F_DISK_SYNC) {
+        const int f = open(im.staged.c_str(), O_RDONLY | O_CLOEXEC);
+        const bool synced = f >= 0 && fsync(f) == 0;
+        if (f >= 0) close(f);
+        if (!synced) return fail(DM_EIO, "could not fsync the imported copy");
+    }
+    Digest d;
+    memcpy(d.b, im.got, 32);
+    const uint64_t size = (uint64_t)c.seen.st_size;
+    const std::string dst = blob_path(e, d.b);
+    mkdirs(dst);
+    struct stat st;
+    const bool placed = stat(dst.c_str(), &st) != 0;    // already in the disk tier: keep that copy, the staged one goes
+    if (placed) {
+        if (rename(im.staged.c_str(), dst.c_str()) != 0) return fail(DM_EIO, "could not move the imported copy into the disk tier");
+        im.staged.clear();
+        Blob b;
+        b.digest = d; b.size = size;
+        if (!write_sidecar(dst + ".meta", b)) {
+            unlink(dst.c_str());
+            unlink((dst + ".meta").c_str());
+            return fail(DM_EIO, "could not write the imported blob's sidecar");
+        }
+    }
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(d);
+        if (it == e->blobs.end()) {
+            auto b = std::make_shared<Blob>();
+            b->digest = d; b->size = size;
+            b->on_disk = b->spill_done = true;
+            e->blobs[d] = b;
+        } else if (!it->second->on_disk) {
+            it->second->on_disk = it->second->spill_done = true;
+        }
+    }
+    if (placed) e->st_committed++;
+    return DM_OK;
+}
+
+}  // namespace
+
+static int cache_import_impl(dm_engine *e, const char *const *paths, const uint8_t *expect, const char *const *keys,
+                             uint32_t n, uint32_t flags, uint8_t *digests_out, int32_t *status_out)
+{
+    if (!e || (n && (!paths || !digests_out || !status_out))) return fail(DM_EINVAL, "null argument");
+    if (flags & ~DM_IMP_LINK) return fail(DM_EINVAL, "unknown dm_cache_import flag");
+    for (uint32_t i = 0; i < n; ++i) {
+        if (!paths[i]) return fail(DM_EINVAL, "null path");
+        if (keys && keys[i] && !alias_key_ok(keys[i])) return fail(DM_EINVAL, "alias key must be 1..4096 bytes without control characters");
+    }
+    if (e->cas_dir.empty()) return fail(DM_ESTATE, "dm_cache_import needs a cas_dir");
+    // staged copies of an import that was killed part way would otherwise stay for good on an engine that never
+    // sweeps (one without DM_F_DISK_DIRECT)
+    mkdirs(e->cas_dir + "/incoming/x");
+    sweep_incoming(e->cas_dir + "/incoming");
+    static const uint8_t kZero[32] = {0};
+    std::vector<Check> work;
+    std::vector<Import> imp;
+    std::vector<uint32_t> slot_of(n);
+    {
+        std::unordered_map<std::string, uint32_t> first;       // path and expected digest: a duplicate is imported once
+        for (uint32_t i = 0; i < n; ++i) {
+            const uint8_t *x = expect ? expect + 32ull * i : kZero;
+            std::string key(paths[i]);
+            key.push_back('\0');
+            key.append((const char *)x, 32);
+            auto ins = first.emplace(std::move(key), (uint32_t)work.size());
+            if (ins.second) {
+                work.emplace_back();
+                imp.emplace_back();
+                work.back().known = memcmp(x, kZero, 32) != 0;
+                memcpy(work.back().d.b, x, 32);
+                imp.back().src = paths[i];
+            }
+            slot_of[i] = ins.first->second;
+        }
+    }
+    CheckRun run(e, work.size());
+    run.run(work,
+            [&](Check &c, int *fd, std::string *path) -> int {
+                return import_prepare(e, run, flags, c, imp[&c - work.data()], fd, path);
+            },
+            [&](Check &c, int rc) -> int {
+                Import &im = imp[&c - work.data()];
+                if (rc == 1) rc = import_publish(e, c, im);
+                if (!im.staged.empty()) { unlink(im.staged.c_str()); im.staged.clear(); }
+                return rc;
+            });
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t k = slot_of[i];
+        status_out[i] = work[k].status;
+        const bool has = work[k].status == DM_OK || work[k].status == DM_ECORRUPT;
+        memcpy(digests_out + 32ull * i, has ? imp[k].got : kZero, 32);
+        if (work[k].status == DM_OK && keys && keys[i]) dm_cache_alias_put(e, keys[i], imp[k].got);
+    }
     return DM_OK;
 }
 
@@ -1602,6 +1861,11 @@ int dm_cache_promote(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *
 int dm_cache_verify(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
 {
     return note_err(e, 0, cache_verify_impl(e, digests, n, status_out));
+}
+int dm_cache_import(dm_engine *e, const char *const *paths, const uint8_t *expect, const char *const *keys, uint32_t n,
+                    uint32_t flags, uint8_t *digests_out, int32_t *status_out)
+{
+    return note_err(e, 0, cache_import_impl(e, paths, expect, keys, n, flags, digests_out, status_out));
 }
 int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, uint64_t *sizes_out, uint32_t cap,
                   uint32_t *n_out)

@@ -385,7 +385,7 @@ bool digest_from_hex(const char *hex, uint8_t out[32])
     return true;
 }
 
-static bool alias_key_ok(const char *key)
+bool alias_key_ok(const char *key)
 {
     if (!key || !*key) return false;
     size_t n = 0;

@@ -496,13 +496,13 @@ std::string sidecar_json(const Blob &b)
     return o + "}}\n";
 }
 
-void write_sidecar(const std::string &path, const Blob &b)
+bool write_sidecar(const std::string &path, const Blob &b)
 {
     FILE *f = fopen(path.c_str(), "w");
-    if (!f) return;
+    if (!f) return false;
     const std::string j = sidecar_json(b);
-    fwrite(j.data(), 1, j.size(), f);
-    fclose(f);
+    const bool ok = fwrite(j.data(), 1, j.size(), f) == j.size();
+    return fclose(f) == 0 && ok;
 }
 
 std::string blob_path(const dm_engine *e, const uint8_t d[32])

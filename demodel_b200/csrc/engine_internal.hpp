@@ -1,8 +1,8 @@
 // engine_internal.hpp - types, constants and internal entry points shared by the engine's translation units:
 //   engine_core.cu    extents, ring slabs, CAS commit / eviction, the pump (launch decisions), the disk tier
 //   engine_api.cu     C-ABI: engine lifecycle, streams (ingest, ranges, checkpoint / resume, zero-copy windows),
-//                     promotion of disk-tier blobs back into HBM and checks of disk-tier files (internal streams),
-//                     the listing of the disk tier
+//                     promotion of disk-tier blobs back into HBM, checks of disk-tier files and imports of files from
+//                     outside the cache (internal streams), the listing of the disk tier
 //   engine_cache.cu   C-ABI: hit serving (readers, followers), device-resident ingest, the synthetic generator
 // Not installed, not part of the boundary (that is include/demodel_b200.h).
 #pragma once
@@ -192,9 +192,10 @@ struct Stream {
     uint32_t disk_writes = 0, disk_reads = 0;    // in flight on the disk threads (at most one read)
     bool publishing = false;                     // the final rename / sidecar is running on a disk thread
     bool suspending = false;                     // dm_stream_suspend: no further read-back or launch
-    // dm_cache_verify: a check of a stored file, never a download.  A disk-backed check reads the blob file itself
-    // (fd / path, every byte already written); a tiny one travels in a pack as a hash-only member.  It holds no arena
-    // extent, and its verdict is all it produces: nothing is published, renamed, truncated or unlinked.
+    // dm_cache_verify / dm_cache_import: a check of a stored file, never a download.  A disk-backed check reads the
+    // file itself (fd / path, every byte already written: a blob file, or an import's staged copy); a tiny one travels
+    // in a pack as a hash-only member.  It holds no arena extent, and its verdict is all it produces: nothing is
+    // published, renamed, truncated or unlinked by the stream (an import publishes its copy itself afterwards).
     bool check_only = false;
     // A body announced (Content-Length) as at most tiny_max bytes never takes a ring slab: its bytes gather in this
     // private buffer and go straight into a pack when it finishes.  Anything that needs a real slab (more bytes than
@@ -315,7 +316,7 @@ struct dm_engine {
     std::atomic<bool> ring_starved{false};
     std::mutex slot_mu;              // state / digest slots: a lock of their own, so that opening and closing tiny bodies from
     std::vector<uint32_t> free_slots;                // many threads does not queue on the index lock `mu`
-    size_t promote_reserved = 0;     // slots running dm_cache_promote / dm_cache_verify calls may take (slot_mu)
+    size_t promote_reserved = 0;     // slots running dm_cache_promote / verify / import calls may take (slot_mu)
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp
     std::unordered_map<Digest, std::weak_ptr<Stream>, DigestHash> inflight;   // open streams by expected digest
@@ -463,7 +464,7 @@ int submit_part(dm_engine *e, const std::shared_ptr<Stream> &sp, size_t idx);
 bool range_taken(const Stream *s, uint64_t off, uint64_t len, const Stream::Part *self);
 std::string json_quote(const std::string &v);
 std::string sidecar_json(const Blob &b);
-void write_sidecar(const std::string &path, const Blob &b);
+bool write_sidecar(const std::string &path, const Blob &b);   // false: the sidecar could not be written whole
 std::string blob_path(const dm_engine *e, const uint8_t d[32]);
 std::shared_ptr<Blob> publish(dm_engine *e, const Digest &d, uint64_t size, std::vector<Extent> &ext,
                               std::vector<std::pair<std::string, std::string>> *meta = nullptr);
@@ -497,5 +498,6 @@ void drop_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, bool release_s
 int ensure_ingest_scratch(dm_engine *e, uint32_t n);
 void alias_load(dm_engine *e);                // dm_engine_create: replay <cas_dir>/aliases.log
 bool digest_from_hex(const char *hex, uint8_t out[32]);
+bool alias_key_ok(const char *key);           // 1..4096 bytes without control characters: one line of aliases.log
 
 }  // namespace dmi

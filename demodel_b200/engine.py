@@ -9,13 +9,14 @@ libdemodel_b200.so; nothing here hashes or copies blob bytes on the CPU.
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import Iterable, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
-from ._lib import (DM_ENOENT, DM_ING_FORCE_DEEP, DM_ING_FORCE_WIDE, DM_ING_HASH_ONLY, DM_ING_REPLACE, DM_OK,
-                   DmConfig, DmError, DmStats, check)
+from ._lib import (DM_ENOENT, DM_IMP_LINK, DM_ING_FORCE_DEEP, DM_ING_FORCE_WIDE, DM_ING_HASH_ONLY, DM_ING_REPLACE,
+                   DM_OK, DmConfig, DmError, DmStats, check)
 
 
 def _buf_ptr(buf) -> tuple[C.c_void_p, int]:
@@ -269,6 +270,33 @@ class Engine:
         check(self._lib.dm_cache_list(self._h, _digest_arg(after), digs, sizes, cap, C.byref(n)), "dm_cache_list")
         raw = bytes(digs)
         return [(raw[32 * i:32 * i + 32], sizes[i]) for i in range(n.value)]
+
+    def import_files(self, paths: Sequence[str], expect: Optional[Sequence[Optional[bytes]]] = None,
+                     keys: Optional[Sequence[Optional[str]]] = None, link: bool = False) -> list[tuple[int, bytes]]:
+        """dm_cache_import: hash files already on the host on the GPU and place them in the disk tier.  expect[i] is
+        the SHA-256 paths[i] must hash to, or None when it is not known; keys[i], when not None, is entered in the
+        alias index once entry i is cached.  link=True hard-links instead of copying where it can.  One (status,
+        digest) per path: DM_OK (digest: its SHA-256), DM_ECORRUPT (digest: what it hashed to), DM_ENOENT, DM_EINVAL
+        (not a regular file), DM_EIO, DM_ECUDA or DM_ENOMEM; the digest is 32 zero bytes for the last five."""
+        paths = [os.fsencode(p) for p in paths]
+        n = len(paths)
+        if expect is not None:
+            expect = list(expect)
+            if len(expect) != n or any(x is not None and len(x) != 32 for x in expect):
+                raise ValueError("expect must hold one 32-byte digest or None per path")
+        if keys is not None:
+            keys = list(keys)
+            if len(keys) != n:
+                raise ValueError("keys must hold one key or None per path")
+        c_paths = (C.c_char_p * max(n, 1))(*paths)
+        rows = b"".join(x if x is not None else bytes(32) for x in expect) if expect is not None else None
+        c_keys = (C.c_char_p * max(n, 1))(*[k.encode() if k is not None else None for k in keys]) if keys is not None else None
+        digs = (C.c_uint8 * (32 * max(n, 1)))()
+        status = (C.c_int32 * max(n, 1))()
+        check(self._lib.dm_cache_import(self._h, c_paths, C.cast(C.c_char_p(rows), C.c_void_p) if rows else None,
+                                        c_keys, n, DM_IMP_LINK if link else 0, digs, status), "dm_cache_import")
+        raw = bytes(digs)
+        return [(status[i], raw[32 * i:32 * i + 32]) for i in range(n)]
 
     # -- URL-keyed requests (the OnRequest hook is handed a URL) -----------------------
     def alias_put(self, key: str, digest: bytes) -> None:

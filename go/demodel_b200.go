@@ -478,6 +478,74 @@ func (p *Pool) Verify(digests [][32]byte) ([]int, error) {
 	return status, first
 }
 
+// ImportFile is one file for Pool.Import.
+type ImportFile struct {
+	Path   string    // a regular file; symlinks are followed
+	Digest *[32]byte // its SHA-256 when the layout names it (an Ollama blob, a HuggingFace LFS blob), else nil
+	Key    string    // a URL to enter in the alias index once the file is cached ("" for none)
+}
+
+// Import seeds the disk tier from files already on the host (dm_cache_import): each file is staged under
+// <CacheDir>/incoming/, hashed on the GPU and renamed into the tier, the engines in parallel.  A file with a known
+// digest goes to the engine that owns that digest; a file without one goes to engine 0, with its key, as a body
+// whose digest is unknown is homed by its URL and found by HitURL on every engine.  link hard-links files into the
+// cache where it can instead of copying them.  It blocks until every file has a status: 0 (DM_OK, in the disk tier
+// now, digests[i] its SHA-256) or a negative dm_err - DM_ECORRUPT (it does not hash to Digest; digests[i] is what it
+// hashed to), DM_ENOENT, DM_EINVAL (not a regular file), DM_EIO, DM_ECUDA or DM_ENOMEM.  Sources are never modified.
+func (p *Pool) Import(files []ImportFile, link bool) ([]int, [][32]byte, error) {
+	status := make([]int, len(files))
+	digests := make([][32]byte, len(files))
+	byEngine := make(map[*C.dm_engine][]int)
+	for i := range files {
+		e := p.engines[0]
+		if files[i].Digest != nil {
+			e = p.engineFor(files[i].Digest)
+		}
+		byEngine[e] = append(byEngine[e], i)
+	}
+	var flags C.uint32_t
+	if link {
+		flags = C.DM_IMP_LINK
+	}
+	errs := make(chan error, len(byEngine))
+	for e, idx := range byEngine {
+		go func(e *C.dm_engine, idx []int) {
+			paths := make([]*C.char, len(idx)) // C strings: a Go slice of C pointers may be passed to C
+			keys := make([]*C.char, len(idx))
+			expect := make([][32]byte, len(idx))
+			for k, i := range idx {
+				paths[k] = C.CString(files[i].Path)
+				if files[i].Key != "" {
+					keys[k] = C.CString(files[i].Key)
+				}
+				if files[i].Digest != nil {
+					expect[k] = *files[i].Digest
+				}
+			}
+			out := make([][32]byte, len(idx))
+			st := make([]C.int32_t, len(idx))
+			err := check(e, 0, C.dm_cache_import(e, (**C.char)(unsafe.Pointer(&paths[0])), (*C.uint8_t)(unsafe.Pointer(&expect[0][0])),
+				(**C.char)(unsafe.Pointer(&keys[0])), C.uint32_t(len(idx)), flags, (*C.uint8_t)(unsafe.Pointer(&out[0][0])), &st[0]))
+			for k, i := range idx {
+				status[i] = int(st[k])
+				digests[i] = out[k]
+				C.free(unsafe.Pointer(paths[k]))
+				if keys[k] != nil {
+					C.free(unsafe.Pointer(keys[k]))
+				}
+			}
+			errs <- err
+		}(e, idx)
+	}
+	var first error
+	for range byEngine {
+		if err := <-errs; err != nil && first == nil {
+			first = err
+		}
+	}
+	return status, digests, first
+}
+
 // List returns up to limit blobs of the disk tier of every engine (dm_cache_list), merged in ascending digest order,
 // strictly after `after` (nil: from the start), with their sizes.  Fewer than limit entries means the listing is
 // complete; the next page starts after the last digest returned.

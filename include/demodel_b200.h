@@ -49,7 +49,8 @@ typedef enum dm_err {
     DM_EIO       = -6,   /* on-disk CAS tier I/O error */
     DM_ENODEV    = -7,   /* no CUDA device / device ordinal out of range */
     DM_ERANGE    = -8,   /* offset beyond blob end */
-    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote, dm_cache_verify) */
+    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote, dm_cache_verify), or a file
+                          * to import does not hash to its expected digest (dm_cache_import) */
 } dm_err;
 
 typedef struct dm_engine dm_engine;   /* opaque; owned by caller between create/destroy */
@@ -280,6 +281,43 @@ int dm_cache_verify(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *s
  * Host code only: "check the whole tier" is dm_cache_list, then dm_cache_verify on each page. */
 int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, uint64_t *sizes_out,
                   uint32_t cap, uint32_t *n_out);
+/* dm_cache_import flags */
+#define DM_IMP_LINK 0x1u   /* hard-link instead of copy when the source is on cas_dir's filesystem */
+/* Seed the disk tier from files already on the host (a HuggingFace hub cache, an Ollama models directory, a copy of
+ * another node's cache): each file is hashed on the GPU and placed at <cas_dir>/blobs/sha256/<aa>/<hex>.
+ *   paths[i]     a regular file; symlinks are followed (HuggingFace snapshots are symlinks into blobs/)
+ *   expect       NULL, or n x 32 bytes: row i is the SHA-256 paths[i] must hash to, all zero when it is not known
+ *   keys         NULL, or n nullable strings: when entry i ends DM_OK, keys[i] is entered in the alias index under its
+ *                digest exactly as dm_cache_alias_put does, on this engine (the one that now holds the blob)
+ *   flags        DM_IMP_LINK: hard-link the source into the cache instead of copying it (falls back to a copy when
+ *                the link fails with EXDEV or EPERM, or when the source was renamed over after it was opened).  The
+ *                tier file then shares the source's inode: a later in-place
+ *                change of the source changes the cached bytes, which only dm_cache_verify would notice
+ * Each source is first staged as a private file <cas_dir>/incoming/<pid>-<device>-<id>.part (copy_file_range, a
+ * reflink on XFS and btrfs, with a pread / pwrite fall-back), and that file is what the GPU hashes, through the ring as
+ * dm_cache_verify reads a tier file (files of at most 64 KiB share pack DMAs and launches), and what is renamed into
+ * the tier: a source that changes while it is copied cannot put bytes in the tier that were never hashed.  The blob is
+ * given a sidecar with its digest and size and no response headers, and registered as on the disk tier only.
+ * Nothing goes into HBM: hbm_cas_used and the LRU order stay as they are (dm_cache_promote loads blobs later).
+ * Blocks until every status is known.  status_out[i] (digests_out[i] is 32 zero bytes unless stated):
+ *   DM_OK        in the disk tier now, imported or already there; digests_out[i] is its SHA-256.  An entry whose
+ *                digest is known and already on either tier is DM_OK at once: nothing is read, copied or hashed
+ *   DM_ECORRUPT  it does not hash to expect[i]; nothing is cached, digests_out[i] is what it hashed to
+ *   DM_ENOENT    no such file
+ *   DM_EINVAL    not a regular file
+ *   DM_EIO       the source could not be read, or the copy could not be written, renamed or given its sidecar
+ *   DM_ECUDA     a copy or launch failed
+ *   DM_ENOMEM    no stream slot to spare (the budget of dm_cache_promote and dm_cache_verify, shared with them)
+ * After any of these the source is untouched, bytes and inode, and <cas_dir>/incoming/ holds nothing of the call.
+ * Duplicate entries (same path and expect row) are imported once; each gets the status, digest and its own alias.
+ * Threads, slot budget and ring share are dm_cache_verify's.  bytes_hashed and h2d_bytes grow by the bytes hashed,
+ * blobs_committed by the blobs newly placed; bytes_ingested and blobs_mismatched do not move.
+ * Each call first removes the files under <cas_dir>/incoming/ of processes that are gone, as dm_engine_create does
+ * under DM_F_DISK_DIRECT: engines that import must not share a cas_dir across PID namespaces either.
+ * Returns DM_OK once every status is filled; DM_EINVAL on bad arguments (a null path, a key that dm_cache_alias_put
+ * would refuse, an unknown flag); DM_ESTATE without cas_dir. */
+int dm_cache_import(dm_engine *e, const char *const *paths, const uint8_t *expect, const char *const *keys,
+                    uint32_t n, uint32_t flags, uint8_t *digests_out, int32_t *status_out);
 /* Request coalescing: the blob is not cached yet but another connection is
  * ingesting it right now (a stream opened with this expected digest).  The
  * reader follows that body out of HBM: dm_cache_read blocks until bytes past
