@@ -74,6 +74,22 @@ class DmLayer(C.Structure):
     _fields_ = [("digest", C.c_uint8 * 32), ("size", C.c_uint64), ("media_type", C.c_char * 96)]
 
 
+class DmDiskUsage(C.Structure):
+    _fields_ = [
+        ("struct_size", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("limit_bytes", C.c_uint64),
+        ("used_bytes", C.c_uint64),
+        ("blob_files", C.c_uint64),
+        ("blob_bytes", C.c_uint64),
+        ("staging_bytes", C.c_uint64),
+        ("partial_bytes", C.c_uint64),
+        ("evicted_files", C.c_uint64),
+        ("evicted_bytes", C.c_uint64),
+        ("refused", C.c_uint64),
+    ]
+
+
 class DmCheckpoint(C.Structure):
     _fields_ = [("h", C.c_uint32 * 8), ("bytes", C.c_uint64), ("abi", C.c_uint32), ("reserved", C.c_uint32)]
 
@@ -116,6 +132,8 @@ SIGNATURES = {
     "dm_cache_list": (C.c_int, [_P, _P, _P, _U64P, C.c_uint32, C.POINTER(C.c_uint32)]),
     "dm_cache_import": (C.c_int, [_P, C.POINTER(C.c_char_p), _P, C.POINTER(C.c_char_p), C.c_uint32, C.c_uint32, _P,
                                   C.POINTER(C.c_int32)]),
+    "dm_cache_set_disk_limit": (C.c_int, [_P, C.c_uint64]),
+    "dm_cache_disk_usage": (C.c_int, [_P, C.POINTER(DmDiskUsage)]),
     "dm_cache_follow": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_alias_put": (C.c_int, [_P, C.c_char_p, _P]),
     "dm_cache_alias_get": (C.c_int, [_P, C.c_char_p, _P]),

@@ -47,6 +47,10 @@ bool numa_cpus_of_device(int device, cpu_set_t *set, int *node_out)
     return n_set > 0;
 }
 
+}  // namespace
+
+namespace dmi {
+
 // Files of disk-backed streams are named <pid>-<device>-<id>.part: remove those of processes that are gone, and
 // leave every live process's alone (other engines may share the directory).
 void sweep_incoming(const std::string &dir)
@@ -63,7 +67,7 @@ void sweep_incoming(const std::string &dir)
     closedir(d);
 }
 
-}  // namespace
+}  // namespace dmi
 
 extern "C" {
 
@@ -393,7 +397,10 @@ int dm_engine_stats(dm_engine *e, dm_stats *o)
 // `followable`: index the stream by its expected digest so that dm_cache_follow can attach to it.  A
 // resumed stream is registered by dm_stream_resume itself, and only when it starts at byte 0: a follower
 // reads from offset 0, and nothing before resume_base is ever written.
-static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, bool followable)
+// `saved`: bytes of this body already counted in the disk tier (a saved download being resumed): a disk-backed stream
+// makes room only for the rest of its size_hint.
+static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, bool followable,
+                            uint64_t saved = 0)
 {
     if (!e || !id) return fail(DM_EINVAL, "null argument");
     auto sp = std::make_shared<Stream>();
@@ -416,16 +423,20 @@ static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t siz
         }
         sp->verify_only = true;
     }
-    if (sp->verify_only && (e->cfg.flags & DM_F_DISK_DIRECT)) {      // kept after all: in a file of the disk tier
+    // kept after all: in a file of the disk tier, when the disk-tier limit leaves room for the announced size (a body
+    // of unknown size is charged as it grows); otherwise it stays verify-only: verified, not cached
+    sp->path = incoming_path(e, sp->id);
+    if (sp->verify_only && (e->cfg.flags & DM_F_DISK_DIRECT) && tier_stage(e, sp->path, size_hint, saved)) {
         sp->disk = true;
-        sp->path = incoming_path(e, sp->id);
         sp->fd = open(sp->path.c_str(), O_CREAT | O_TRUNC | O_RDWR | O_CLOEXEC, 0644);
         if (sp->fd < 0) {
+            tier_unstage(e, sp->path);
             std::lock_guard<std::mutex> g2(e->slot_mu);
             e->free_slots.push_back(sp->slot);
             return fail(DM_EIO, "could not create the stream's file under <cas_dir>/incoming");
         }
     }
+    if (!sp->disk) sp->path.clear();
     if (size_hint && !sp->verify_only) {
         cudaSetDevice(e->device);
         std::lock_guard<std::mutex> g(sp->mu);
@@ -630,19 +641,21 @@ static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out)
     return read_chain_state(e, s->slot, s->hash_issued, out->h);
 }
 
-static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id);
+static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id,
+                              uint64_t saved = 0);
 int dm_stream_resume(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id)
 {
     return note_err(e, 0, stream_resume_impl(e, ck, expect, size_hint, id));
 }
-static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id)
+static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id,
+                              uint64_t saved)
 {
     if (!e || !ck || !id) return fail(DM_EINVAL, "null argument");
     if (ck->abi != DM_ABI_VERSION || (ck->bytes & 63)) return fail(DM_EINVAL, "bad checkpoint");
     // Not followable while it is being set up (a follower attaching now would read [0, ck->bytes) out of an
     // extent nothing has been written to), and never when it starts past byte 0: the prefix may not be
     // re-supplied at all, so there is nothing to serve from offset 0.
-    int rc = stream_open_impl(e, expect, size_hint, id, false);
+    int rc = stream_open_impl(e, expect, size_hint, id, false, saved);
     if (rc != DM_OK) return rc;
     auto sp = find_stream(e, *id);
     if (!sp) return fail(DM_ESTATE, "stream closed while resuming");
@@ -666,7 +679,7 @@ static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8
         if (err != cudaSuccess) {
             // nothing of this stream is in flight yet: give back its extent, state slot and id
             s->st = St::Aborted;
-            if (s->disk) { close(s->fd); s->fd = -1; unlink(s->path.c_str()); }
+            if (s->disk) { close(s->fd); s->fd = -1; unlink(s->path.c_str()); tier_unstage(e, s->path); }
             g.unlock();
             free_extents(e, s->extents);
             drop_stream(e, sp, true);
@@ -703,7 +716,6 @@ std::string partial_base(const dm_engine *e, const uint8_t d[32]) { return e->ca
 
 static int stream_abort_impl(dm_engine *e, uint64_t id);
 static int stream_checkpoint_impl(dm_engine *e, uint64_t id, dm_checkpoint *out);
-static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8_t expect[32], uint64_t size_hint, uint64_t *id);
 
 // dm_stream_suspend of a disk-backed stream: no wait for the hash, no copy.  The state at the hashed position H
 // is saved with H and C (the contiguous written prefix, rounded down to 64); the file, cut to C, is renamed.
@@ -769,6 +781,7 @@ static int suspend_disk(dm_engine *e, const std::shared_ptr<Stream> &sp, uint64_
         unlink((base + ".ckpt.tmp").c_str());
         if (moved) rename((base + ".part").c_str(), path.c_str());     // the stream keeps its file
         if (!fresh && e->n_suspended) e->n_suspended--;               // the older record went with the attempt
+        tier_placed(e, s->expect, true, nullptr, false);
         std::unique_lock<std::mutex> g(s->mu);
         unsuspend(g);
         return fail(DM_EIO, "could not save the checkpoint under <cas_dir>/partial (the stream is still open)");
@@ -779,12 +792,15 @@ static int suspend_disk(dm_engine *e, const std::shared_ptr<Stream> &sp, uint64_
         s->fd = -1;
         s->path.clear();
     }
+    tier_unstage(e, path);                               // its bytes moved from incoming/ to partial/
+    tier_placed(e, s->expect, true, nullptr, true);
     if (fresh) e->n_suspended++;
     stream_abort_impl(e, s->id);                         // releases the id, the state slot and the staged slabs
     if (resume_from) *resume_from = saved;
     return DM_OK;
 }
 
+static int stream_suspend_saving(dm_engine *e, const std::shared_ptr<Stream> &sp, uint64_t *resume_from);
 static int stream_suspend_impl(dm_engine *e, uint64_t id, uint64_t *resume_from)
 {
     if (!e) return fail(DM_EINVAL, "null argument");
@@ -792,11 +808,23 @@ static int stream_suspend_impl(dm_engine *e, uint64_t id, uint64_t *resume_from)
     if (e->cas_dir.empty()) return fail(DM_ESTATE, "dm_stream_suspend needs a disk tier (cas_dir)");
     auto sp = find_stream(e, id);
     if (!sp) return fail(DM_EINVAL, "unknown stream id");
+    {
+        std::lock_guard<std::mutex> g(sp->mu);
+        if (!sp->has_expect) return fail(DM_ESTATE, "only a stream opened with an expected digest can be suspended (the digest names the saved files)");
+    }
+    tier_pin(e, sp->expect, true);                       // the saved download it writes is not a victim meanwhile
+    const int rc = stream_suspend_saving(e, sp, resume_from);
+    tier_unpin(e, sp->expect, true);
+    return rc;
+}
+
+static int stream_suspend_saving(dm_engine *e, const std::shared_ptr<Stream> &sp, uint64_t *resume_from)
+{
     Stream *s = sp.get();
+    const uint64_t id = s->id;
     bool disk;
     {
         std::lock_guard<std::mutex> g(s->mu);
-        if (!s->has_expect) return fail(DM_ESTATE, "only a stream opened with an expected digest can be suspended (the digest names the saved files)");
         if (s->verify_only && !s->disk) return fail(DM_ESTATE, "a verify-only stream retains no bytes to save");
         const bool whole = s->resume_base == 0 ||
                            (s->prefix_cover.size() == 1 && s->prefix_cover.begin()->first == 0 &&
@@ -808,11 +836,14 @@ static int stream_suspend_impl(dm_engine *e, uint64_t id, uint64_t *resume_from)
     dm_checkpoint ck;
     int rc = stream_checkpoint_impl(e, id, &ck);        // every whole block received in order is hashed now
     if (rc != DM_OK) return rc;
+    TierRes res;
+    if (!tier_reserve(e, ck.bytes + sizeof(SavedCkpt), true, &res))
+        return fail(DM_ENOMEM, "no room under the disk-tier limit for the saved download (the stream is still open)");
     std::vector<Extent> ext;
     uint64_t hint;
     {
         std::lock_guard<std::mutex> g(s->mu);
-        if (s->st != St::Open) return fail(DM_ESTATE, "stream closed during suspend");
+        if (s->st != St::Open) { tier_release(e, res); return fail(DM_ESTATE, "stream closed during suspend"); }
         ext = s->extents;
         hint = s->size_hint;
         s->follow_reads++;                               // pins the extents against abort / completion while they are copied out
@@ -847,19 +878,34 @@ static int stream_suspend_impl(dm_engine *e, uint64_t id, uint64_t *resume_from)
         unlink((base + ".ckpt.tmp").c_str());
         struct stat st;
         if (!fresh && stat((base + ".ckpt").c_str(), &st) != 0 && e->n_suspended) e->n_suspended--;    // the older record went with the attempt
+        tier_placed(e, s->expect, true, &res, false);    // (what is left of an older record, if anything)
         return fail(DM_EIO, "could not save the checkpoint under <cas_dir>/partial (the stream is still open)");
     }
+    tier_placed(e, s->expect, true, &res, true);
     if (fresh) e->n_suspended++;
     stream_abort_impl(e, id);                            // releases the id, the state slot and the extent
     if (resume_from) *resume_from = ck.bytes;
     return DM_OK;
 }
 
+static int resume_saved_pinned(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, uint64_t *resume_from);
 static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, uint64_t *resume_from)
 {
     if (!e || !expect || !id) return fail(DM_EINVAL, "null argument");
     if (resume_from) *resume_from = 0;
     if (e->cas_dir.empty()) return DM_ENOENT;
+    Digest d;
+    memcpy(d.b, expect, 32);
+    tier_pin(e, d, true);                                // the saved download being taken over is not a victim
+    const int rc = resume_saved_pinned(e, expect, size_hint, id, resume_from);
+    tier_unpin(e, d, true);
+    return rc;
+}
+
+static int resume_saved_pinned(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, uint64_t *resume_from)
+{
+    Digest dg;
+    memcpy(dg.b, expect, 32);
     const std::string base = partial_base(e, expect);
     SavedCkpt rec;
     uint64_t saved;                                      // bytes in the .part: == rec.bytes, or more for a disk-backed stream's record
@@ -878,6 +924,7 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
             memcmp(rec.expect, expect, 32) != 0) {
             unlink((base + ".ckpt").c_str()); unlink((base + ".part").c_str());
             if (e->n_suspended) e->n_suspended--;
+            tier_forget(e, dg, true);
             return fail(DM_EIO, "saved checkpoint is damaged or from another ABI: discarded");
         }
     }
@@ -885,7 +932,7 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
     memset(&ck, 0, sizeof ck);
     memcpy(ck.h, rec.h, sizeof ck.h);
     ck.bytes = rec.bytes; ck.abi = DM_ABI_VERSION;
-    int rc = stream_resume_impl(e, &ck, expect, size_hint ? size_hint : rec.size_hint, id);
+    int rc = stream_resume_impl(e, &ck, expect, size_hint ? size_hint : rec.size_hint, id, saved);
     if (rc != DM_OK) return rc;
     // Re-supply the saved prefix [0, rec.bytes) (cached, not re-hashed) and the saved bytes past it (hashed) through
     // the ordinary range path: ring -> DMA -> extent, or ring -> file.  A blob too large for the arena continues
@@ -913,6 +960,7 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
                 if (rec.bytes) add_interval(s->prefix_cover, 0, rec.bytes);
                 s->dma_issued = s->landed = s->received = saved;
                 disk_feed(e, sp);
+                tier_stage_grow(e, s->path, saved);      // its bytes moved from partial/ back to incoming/
             }
         }
     }
@@ -941,6 +989,7 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
     unlink((base + ".ckpt").c_str());                    // the stream owns the download again
     unlink((base + ".part").c_str());
     if (e->n_suspended) e->n_suspended--;
+    tier_forget(e, dg, true);
     if (resume_from) *resume_from = saved;
     return DM_OK;
 }
@@ -1094,7 +1143,7 @@ static int stream_abort_impl(dm_engine *e, uint64_t id)
             free_now = s->jobs_inflight == 0;
             s->cv.wait(g, [&] { return s->disk_writes == 0 && s->disk_reads == 0 && !s->publishing; });
             if (s->fd >= 0) { close(s->fd); s->fd = -1; }
-            if (!s->path.empty() && !s->check_only) unlink(s->path.c_str());
+            if (!s->path.empty() && !s->check_only) { unlink(s->path.c_str()); tier_unstage(e, s->path); }
         }
         if (!s->staged.empty()) {            // their DMAs may be in flight: drain before the ring reuses them
             cudaSetDevice(e->device);
@@ -1186,7 +1235,7 @@ void drop_corrupt(dm_engine *e, const Digest &d, const struct stat &seen)
     const bool exists = stat(path.c_str(), &now) == 0;
     const bool same = exists && now.st_dev == seen.st_dev && now.st_ino == seen.st_ino;
     if (same) { unlink(path.c_str()); unlink((path + ".meta").c_str()); }
-    if (!exists || same) forget_disk_copy(e, d, nullptr);
+    if (!exists || same) { tier_forget(e, d); forget_disk_copy(e, d, nullptr); }
 }
 
 // The promotion ended without a verdict on the file (no slot or room, a failed read, copy or launch): take back the
@@ -1359,11 +1408,16 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
         flush();
         for (Promotion *p : open) p->status = promote_verdict(e, *p);
     };
+    for (Promotion &p : work) tier_pin(e, p.d);        // held by this call: not disk-tier victims until it returns
     std::vector<std::thread> th;
     for (size_t t = 1; t < nthreads; ++t) th.emplace_back(loader);
     if (nthreads) loader();
     for (auto &t : th) t.join();
     { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved -= budget; }
+    for (Promotion &p : work) {
+        if (p.status == DM_OK) tier_touch(e, p.d);
+        tier_unpin(e, p.d);
+    }
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
     return DM_OK;
 }
@@ -1583,6 +1637,7 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
         }
     }
     CheckRun run(e, work.size());
+    for (Check &c : work) tier_pin(e, c.d);
     run.run(work,
             [&](Check &c, int *fd, std::string *path) -> int {
                 std::string side;
@@ -1593,6 +1648,7 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
                 return 1;
             },
             [&](Check &c, int rc) -> int { return rc == 1 ? check_verdict(e, c) : rc; });
+    for (Check &c : work) tier_unpin(e, c.d);
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
     return DM_OK;
 }
@@ -1680,6 +1736,11 @@ int import_prepare(dm_engine *e, const CheckRun &run, uint32_t flags, Check &c, 
     if (!S_ISREG(st.st_mode)) { close(src); return fail(DM_EINVAL, "not a regular file"); }
     if (const int b = run.blocked()) { close(src); return b; }
     im.staged = incoming_path(e, e->next_id.fetch_add(1));
+    if (!tier_stage(e, im.staged, (uint64_t)st.st_size)) {
+        close(src);
+        im.staged.clear();
+        return fail(DM_ENOMEM, "no room under the disk-tier limit for the file to import");
+    }
     bool linked = false;
     if (flags & DM_IMP_LINK) {
         // ENOENT: the source was replaced (renamed over) since it was opened, and the file that is open has no name
@@ -1687,6 +1748,7 @@ int import_prepare(dm_engine *e, const CheckRun &run, uint32_t flags, Check &c, 
         linked = linkat(AT_FDCWD, im.src, AT_FDCWD, im.staged.c_str(), AT_SYMLINK_FOLLOW) == 0;
         if (!linked && errno != EXDEV && errno != EPERM && errno != ENOENT) {
             close(src);
+            tier_unstage(e, im.staged);
             im.staged.clear();
             return fail(DM_EIO, "could not link the file into <cas_dir>/incoming");
         }
@@ -1700,6 +1762,7 @@ int import_prepare(dm_engine *e, const CheckRun &run, uint32_t flags, Check &c, 
     }
     if (rc != DM_OK) {
         unlink(im.staged.c_str());
+        tier_unstage(e, im.staged);
         im.staged.clear();
         return rc;
     }
@@ -1725,18 +1788,31 @@ int import_publish(dm_engine *e, Check &c, Import &im)
     const uint64_t size = (uint64_t)c.seen.st_size;
     const std::string dst = blob_path(e, d.b);
     mkdirs(dst);
+    struct TierHold {                                    // not a disk-tier victim while it is placed
+        dm_engine *e; Digest d;
+        ~TierHold() { tier_unpin(e, d); }
+    } hold{e, d};
+    tier_pin(e, d);
     struct stat st;
     const bool placed = stat(dst.c_str(), &st) != 0;    // already in the disk tier: keep that copy, the staged one goes
     if (placed) {
-        if (rename(im.staged.c_str(), dst.c_str()) != 0) return fail(DM_EIO, "could not move the imported copy into the disk tier");
-        im.staged.clear();
         Blob b;
         b.digest = d; b.size = size;
+        TierRes res;
+        if (!tier_stage_to_blob(e, im.staged, size, sidecar_json(b).size(), &res))
+            return fail(DM_ENOMEM, "no room under the disk-tier limit for the imported file");
+        if (rename(im.staged.c_str(), dst.c_str()) != 0) {
+            tier_release(e, res);
+            return fail(DM_EIO, "could not move the imported copy into the disk tier");
+        }
+        im.staged.clear();
         if (!write_sidecar(dst + ".meta", b)) {
             unlink(dst.c_str());
             unlink((dst + ".meta").c_str());
+            tier_release(e, res);
             return fail(DM_EIO, "could not write the imported blob's sidecar");
         }
+        tier_placed(e, d, false, &res, true);
     }
     {
         std::lock_guard<std::mutex> g(e->mu);
@@ -1800,7 +1876,7 @@ static int cache_import_impl(dm_engine *e, const char *const *paths, const uint8
             [&](Check &c, int rc) -> int {
                 Import &im = imp[&c - work.data()];
                 if (rc == 1) rc = import_publish(e, c, im);
-                if (!im.staged.empty()) { unlink(im.staged.c_str()); im.staged.clear(); }
+                if (!im.staged.empty()) { unlink(im.staged.c_str()); tier_unstage(e, im.staged); im.staged.clear(); }
                 return rc;
             });
     for (uint32_t i = 0; i < n; ++i) {
@@ -1853,7 +1929,56 @@ static int cache_list_impl(dm_engine *e, const uint8_t after[32], uint8_t *diges
     return DM_OK;
 }
 
+// ---- disk-tier limit (dm_cache_set_disk_limit, dm_cache_disk_usage) ---------------------------------------------
+// The bookkeeping is in engine_core.cu (struct DiskTier); this builds the index on the first limit and evicts down.
+static int cache_set_disk_limit_impl(dm_engine *e, uint64_t limit_bytes)
+{
+    if (!e) return fail(DM_EINVAL, "null argument");
+    if (e->cas_dir.empty()) return fail(DM_ESTATE, "dm_cache_set_disk_limit needs a disk tier (cas_dir)");
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    DiskTier &T = e->tier;
+    if (limit_bytes == 0) {                              // off: nothing is tracked, touched or reserved any more
+        T.on = false;
+        T.limit = 0;
+        T.blobs.clear(); T.saved.clear(); T.order.clear(); T.staging.clear();
+        T.blob_bytes = T.partial_bytes = T.staging_bytes = T.reserved_blob = T.reserved_partial = 0;
+        e->tier_on.store(false, std::memory_order_release);
+        return DM_OK;
+    }
+    if (!T.on) {
+        mkdirs(e->cas_dir + "/incoming/x");
+        tier_build(e);
+        e->tier_on.store(true, std::memory_order_release);
+    }
+    T.limit = limit_bytes;
+    tier_make_room(e, 0, true);                          // down to the limit, or to what is pinned
+    return DM_OK;
+}
+
+static int cache_disk_usage_impl(dm_engine *e, dm_disk_usage *out)
+{
+    if (!e || !out) return fail(DM_EINVAL, "null argument");
+    if (out->struct_size != sizeof(dm_disk_usage)) return fail(DM_EINVAL, "dm_disk_usage has the wrong struct_size");
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    const DiskTier &T = e->tier;
+    memset(out, 0, sizeof *out);
+    out->struct_size = sizeof *out;
+    out->evicted_files = T.evicted_files;
+    out->evicted_bytes = T.evicted_bytes;
+    out->refused = T.refused;
+    if (!T.on) return DM_OK;
+    out->limit_bytes = T.limit;
+    out->blob_files = T.blobs.size();
+    out->blob_bytes = T.blob_bytes + T.reserved_blob;
+    out->staging_bytes = T.staging_bytes;
+    out->partial_bytes = T.partial_bytes + T.reserved_partial;
+    out->used_bytes = out->blob_bytes + out->staging_bytes + out->partial_bytes;
+    return DM_OK;
+}
+
 // ---- exported wrappers: file the error text under the stream id (dm_error_detail) ----
+int dm_cache_set_disk_limit(dm_engine *e, uint64_t limit_bytes) { return note_err(e, 0, cache_set_disk_limit_impl(e, limit_bytes)); }
+int dm_cache_disk_usage(dm_engine *e, dm_disk_usage *out) { return note_err(e, 0, cache_disk_usage_impl(e, out)); }
 int dm_cache_promote(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
 {
     return note_err(e, 0, cache_promote_impl(e, digests, n, status_out));

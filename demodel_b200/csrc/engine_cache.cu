@@ -43,8 +43,11 @@ static int cache_open_impl(dm_engine *e, const uint8_t digest[32], uint64_t *rea
     }
     if (!r->blob) {
         if (e->cas_dir.empty()) return DM_ENOENT;
+        tier_pin(e, d);                                  // an open disk reader: not a disk-tier victim until closed
         r->fd = open(blob_path(e, digest).c_str(), O_RDONLY);
-        if (r->fd < 0) return DM_ENOENT;
+        if (r->fd < 0) { tier_unpin(e, d); return DM_ENOENT; }
+        r->disk_digest = d;
+        tier_touch(e, d);
         struct stat st;
         fstat(r->fd, &st);
         r->size = (uint64_t)st.st_size;
@@ -295,7 +298,7 @@ static int cache_close_impl(dm_engine *e, uint64_t reader)
         std::lock_guard<std::mutex> g(e->mu);
         r->blob->readers--;
     }
-    if (r->fd >= 0) close(r->fd);
+    if (r->fd >= 0) { close(r->fd); tier_unpin(e, r->disk_digest); }
     return DM_OK;
 }
 
@@ -331,6 +334,7 @@ static int cache_evict_impl(dm_engine *e, const uint8_t digest[32])
     memcpy(d.b, digest, 32);
     std::shared_ptr<Blob> b;
     std::vector<Extent> ext;
+    bool touch = false;
     {
         std::lock_guard<std::mutex> g(e->mu);
         auto it = e->blobs.find(d);
@@ -341,7 +345,9 @@ static int cache_evict_impl(dm_engine *e, const uint8_t digest[32])
         lru_drop(e, b.get());
         ext.swap(b->extents);                       // under the lock (see evict_for)
         if (!b->on_disk) e->blobs.erase(it);
+        else touch = true;
     }
+    if (touch) tier_touch(e, d);                    // leaving HBM is its last use
     free_extents(e, ext);
     return DM_OK;
 }

@@ -27,6 +27,8 @@
 // start.go:197-200 (hit serving); see include/demodel_b200.h.
 #include "engine_internal.hpp"
 
+#include <dirent.h>
+
 #if defined(__x86_64__)
 #include <emmintrin.h>
 #endif
@@ -149,6 +151,7 @@ bool evict_for(dm_engine *e, uint64_t need)
     for (;;) {
         std::shared_ptr<Blob> victim;
         std::vector<Extent> ext;
+        bool touch = false;
         {
             std::lock_guard<std::mutex> g(e->mu);
             for (Blob *b = e->lru_head; b; b = b->lru_next) {
@@ -163,7 +166,9 @@ bool evict_for(dm_engine *e, uint64_t need)
             lru_drop(e, victim.get());
             ext.swap(victim->extents);          // taken under the lock: a re-publish may install new ones at once
             if (!victim->on_disk) e->blobs.erase(victim->digest);
+            else touch = true;
         }
+        if (touch) tier_touch(e, victim->digest);     // leaving HBM is its last use
         free_extents(e, ext);
         std::lock_guard<std::mutex> g(e->arena_mu);
         uint64_t off;
@@ -1155,6 +1160,361 @@ bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int 
     return ok;
 }
 
+// ---- disk-tier limit (dm_cache_set_disk_limit) -------------------------------------------------------------------
+// Host bookkeeping only: which entries exist, their bytes and their order.  Every placement reserves its bytes before
+// they reach the disk, and a reservation evicts unpinned entries, least recently used first, until it fits.
+
+static std::string tier_saved_base(const dm_engine *e, const Digest &d) { return e->cas_dir + "/partial/" + hex_of(d.b, 32); }
+
+static uint64_t file_size(const std::string &path, struct stat *out = nullptr)
+{
+    struct stat st;
+    if (stat(path.c_str(), &st) != 0 || !S_ISREG(st.st_mode)) return 0;
+    if (out) *out = st;
+    return (uint64_t)st.st_size;
+}
+
+static int64_t stamp_of(const struct stat &st) { return (int64_t)st.st_mtim.tv_sec * 1000000000 + st.st_mtim.tv_nsec; }
+
+// tier_mu held: `k` becomes the most recently used entry; a blob's file gets the time as its mtime.
+static void tier_rank(dm_engine *e, const TierKey &k, TierEntry &t, bool write_mtime)
+{
+    DiskTier &T = e->tier;
+    if (t.seq) T.order.erase(t.seq);
+    t.seq = ++T.seq;
+    T.order.emplace(t.seq, k);
+    if (!write_mtime || k.saved || t.linked) return;
+    struct timespec now;
+    clock_gettime(CLOCK_REALTIME, &now);
+    const int64_t ns = std::max<int64_t>((int64_t)now.tv_sec * 1000000000 + now.tv_nsec, T.last_stamp + 1);
+    T.last_stamp = ns;
+    const struct timespec ts[2] = {{0, UTIME_OMIT}, {(time_t)(ns / 1000000000), (long)(ns % 1000000000)}};
+    utimensat(AT_FDCWD, blob_path(e, k.d.b).c_str(), ts, 0);
+}
+
+// tier_mu held: drop the entry from the index (its files are gone or going).
+static void tier_erase(dm_engine *e, const Digest &d, bool saved)
+{
+    DiskTier &T = e->tier;
+    auto &m = saved ? T.saved : T.blobs;
+    auto it = m.find(d);
+    if (it == m.end()) return;
+    (saved ? T.partial_bytes : T.blob_bytes) -= it->second.bytes;
+    T.order.erase(it->second.seq);
+    m.erase(it);
+}
+
+// tier_mu held: (re)enter the files of `d` at their current st_size.
+static void tier_enter(dm_engine *e, const Digest &d, bool saved, bool use)
+{
+    DiskTier &T = e->tier;
+    uint64_t bytes;
+    struct stat st{};
+    if (saved) {                                // either file alone is counted (and evicted) too: a record being rewritten
+        const std::string base = tier_saved_base(e, d);
+        struct stat part{};
+        bytes = file_size(base + ".ckpt", &st) + file_size(base + ".part", &part);
+        if (!S_ISREG(st.st_mode)) st = part;
+    } else {
+        const std::string path = blob_path(e, d.b);
+        bytes = file_size(path, &st);
+        if (bytes || S_ISREG(st.st_mode)) bytes += file_size(path + ".meta");
+    }
+    if (!S_ISREG(st.st_mode)) { tier_erase(e, d, saved); return; }
+    auto &m = saved ? T.saved : T.blobs;
+    auto ins = m.emplace(d, TierEntry{});
+    TierEntry &t = ins.first->second;
+    (saved ? T.partial_bytes : T.blob_bytes) += bytes - t.bytes;
+    t.bytes = bytes;
+    t.linked = !saved && st.st_nlink > 1;
+    if (ins.second || use) tier_rank(e, TierKey{d, saved}, t, use);
+}
+
+static bool tier_pinned(const DiskTier &T, const TierKey &k)
+{
+    const auto &p = k.saved ? T.saved_pins : T.pins;
+    auto it = p.find(k.d);
+    return it != p.end() && it->second > 0;
+}
+
+// tier_mu held: evict unpinned entries until `need` more bytes fit under the limit.  Disk-only entries go first, least
+// recently used first; then the disk copies of HBM-resident blobs (the hot set), in HBM LRU order.  `partial`: evict as
+// far as possible even when that is not enough (a new limit); otherwise nothing goes unless the placement then fits.
+// A blob's index entry is updated under e->mu as the victims are taken; the files are removed afterwards (tier_mu keeps
+// every pinning caller out until then).  A blob whose disk copy goes while it stays in HBM is never spilled again.
+bool tier_make_room(dm_engine *e, uint64_t need, bool partial)
+{
+    DiskTier &T = e->tier;
+    if (!T.on || T.used() + need <= T.limit) return true;
+    const uint64_t over = T.used() + need - T.limit;
+    std::vector<TierKey> victims;
+    uint64_t freed = 0;
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        for (auto &kv : T.order) {
+            if (freed >= over) break;
+            const TierKey &k = kv.second;
+            if (tier_pinned(T, k)) continue;
+            if (!k.saved) {
+                auto it = e->blobs.find(k.d);
+                if (it != e->blobs.end() && it->second->in_hbm) continue;
+            }
+            victims.push_back(k);
+            freed += (k.saved ? T.saved : T.blobs)[k.d].bytes;
+        }
+        for (Blob *b = e->lru_head; b && freed < over; b = b->lru_next) {
+            auto it = T.blobs.find(b->digest);
+            const TierKey k{b->digest, false};
+            if (it == T.blobs.end() || tier_pinned(T, k)) continue;
+            victims.push_back(k);
+            freed += it->second.bytes;
+        }
+        if (freed < over && !partial) return false;
+        for (const TierKey &k : victims) {
+            if (k.saved) continue;
+            auto it = e->blobs.find(k.d);
+            if (it == e->blobs.end()) continue;
+            if (it->second->in_hbm) { it->second->on_disk = false; it->second->spill_done = true; }
+            else e->blobs.erase(it);
+        }
+    }
+    for (const TierKey &k : victims) {
+        uint64_t bytes;
+        if (k.saved) {
+            const std::string base = tier_saved_base(e, k.d);
+            unlink((base + ".ckpt").c_str());            // the record first: a .part without it is never resumed
+            unlink((base + ".part").c_str());
+            if (e->n_suspended) e->n_suspended--;
+            bytes = T.saved[k.d].bytes;
+        } else {
+            const std::string path = blob_path(e, k.d.b);
+            unlink(path.c_str());
+            unlink((path + ".meta").c_str());
+            bytes = T.blobs[k.d].bytes;
+        }
+        T.evicted_files++;
+        T.evicted_bytes += bytes;
+        tier_erase(e, k.d, k.saved);
+    }
+    return T.used() + need <= T.limit;
+}
+
+static void count_down(std::unordered_map<Digest, uint32_t, DigestHash> &m, const Digest &d)
+{
+    auto it = m.find(d);
+    if (it != m.end() && --it->second == 0) m.erase(it);
+}
+
+void tier_pin(dm_engine *e, const Digest &d, bool saved, bool spill)
+{
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    (saved ? e->tier.saved_pins : e->tier.pins)[d]++;
+    if (spill) e->tier.spills[d]++;
+}
+
+void tier_unpin(dm_engine *e, const Digest &d, bool saved, bool spill)
+{
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    count_down(saved ? e->tier.saved_pins : e->tier.pins, d);
+    if (spill) count_down(e->tier.spills, d);
+}
+
+bool tier_reserve(dm_engine *e, uint64_t bytes, bool partial, TierRes *r)
+{
+    *r = TierRes{};
+    if (!e->tier_on.load(std::memory_order_acquire)) return true;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    DiskTier &T = e->tier;
+    if (!T.on) return true;
+    if (!tier_make_room(e, bytes, false)) { T.refused++; return false; }
+    (partial ? T.reserved_partial : T.reserved_blob) += bytes;
+    *r = TierRes{bytes, T.gen, partial};
+    return true;
+}
+
+static void tier_release_locked(dm_engine *e, TierRes &r)
+{
+    DiskTier &T = e->tier;
+    if (r.gen && T.on && r.gen == T.gen) (r.partial ? T.reserved_partial : T.reserved_blob) -= r.bytes;
+    r = TierRes{};
+}
+
+void tier_release(dm_engine *e, TierRes &r)
+{
+    if (!r.gen) return;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    tier_release_locked(e, r);
+}
+
+void tier_placed(dm_engine *e, const Digest &d, bool saved, TierRes *r, bool use)
+{
+    if (!e->tier_on.load(std::memory_order_acquire) && !(r && r->gen)) return;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    if (r) tier_release_locked(e, *r);
+    if (e->tier.on) tier_enter(e, d, saved, use);
+}
+
+void tier_touch(dm_engine *e, const Digest &d)
+{
+    if (!e->tier_on.load(std::memory_order_acquire)) return;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    auto it = e->tier.blobs.find(d);
+    if (e->tier.on && it != e->tier.blobs.end()) tier_rank(e, TierKey{d, false}, it->second, true);
+}
+
+void tier_forget(dm_engine *e, const Digest &d, bool saved)
+{
+    if (!e->tier_on.load(std::memory_order_acquire)) return;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    if (e->tier.on) tier_enter(e, d, saved, false);    // what is there now: another call may have placed files meanwhile
+}
+
+static void tier_charge(DiskTier &T, std::pair<uint64_t, uint64_t> &s, uint64_t reserved, uint64_t written)
+{
+    T.staging_bytes -= std::max(s.first, s.second);
+    s.first = reserved; s.second = written;
+    T.staging_bytes += std::max(s.first, s.second);
+}
+
+bool tier_stage(dm_engine *e, const std::string &path, uint64_t reserve, uint64_t counted)
+{
+    if (!e->tier_on.load(std::memory_order_acquire)) return true;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    DiskTier &T = e->tier;
+    if (!T.on) return true;
+    const uint64_t need = reserve - std::min(reserve, counted);
+    if (need && !tier_make_room(e, need, false)) { T.refused++; return false; }
+    tier_charge(T, T.staging[path], reserve, 0);
+    return true;
+}
+
+void tier_stage_grow(dm_engine *e, const std::string &path, uint64_t written)
+{
+    if (!e->tier_on.load(std::memory_order_acquire)) return;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    DiskTier &T = e->tier;
+    if (!T.on) return;
+    auto &s = T.staging[path];
+    if (written > s.second) tier_charge(T, s, s.first, written);
+}
+
+void tier_unstage(dm_engine *e, const std::string &path)
+{
+    if (!e->tier_on.load(std::memory_order_acquire)) return;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    DiskTier &T = e->tier;
+    auto it = T.staging.find(path);
+    if (it == T.staging.end()) return;
+    tier_charge(T, it->second, 0, 0);
+    T.staging.erase(it);
+}
+
+bool tier_stage_to_blob(dm_engine *e, const std::string &path, uint64_t size, uint64_t side, TierRes *r)
+{
+    *r = TierRes{};
+    if (!e->tier_on.load(std::memory_order_acquire)) return true;
+    std::lock_guard<std::mutex> g(e->tier_mu);
+    DiskTier &T = e->tier;
+    uint64_t granted = 0;                       // room reserved for the body when it was staged
+    auto it = T.staging.find(path);
+    if (it != T.staging.end()) { granted = it->second.first; tier_charge(T, it->second, 0, 0); T.staging.erase(it); }
+    if (!T.on) return true;
+    // A body whose room was reserved up front keeps it: it is placed even when unknown-size bodies have run the tier
+    // over the limit meanwhile (its sidecar then adds to that overshoot), unless the limit has since been lowered below
+    // what it needs.  Anything else must fit now.
+    const uint64_t bytes = size + side;
+    if (!tier_make_room(e, bytes, false) && (granted < size || bytes > T.limit)) { T.refused++; return false; }
+    T.reserved_blob += bytes;
+    *r = TierRes{bytes, T.gen, false};
+    return true;
+}
+
+// tier_mu held: the one walk of blobs/, incoming/ and partial/ that builds the index.  Removes spill leftovers
+// (<hex>.part under blobs/ with no spill of this engine running), sidecars without their blob and the incoming/ files
+// of processes that are gone.  Entries are ranked by mtime.
+void tier_build(dm_engine *e)
+{
+    DiskTier &T = e->tier;
+    T.blobs.clear(); T.saved.clear(); T.order.clear(); T.staging.clear();
+    T.blob_bytes = T.partial_bytes = T.staging_bytes = T.reserved_blob = T.reserved_partial = 0;
+    T.gen++;
+    std::vector<std::pair<int64_t, TierKey>> ranked;
+    const std::string root = e->cas_dir + "/blobs/sha256/";
+    for (int p = 0; p < 256; ++p) {
+        char aa[3];
+        snprintf(aa, sizeof aa, "%02x", p);
+        const std::string dir = root + aa + "/";
+        DIR *d = opendir(dir.c_str());
+        if (!d) continue;
+        std::vector<std::string> names;
+        while (struct dirent *de = readdir(d)) if (de->d_name[0] != '.') names.emplace_back(de->d_name);
+        closedir(d);
+        std::unordered_map<Digest, uint64_t, DigestHash> metas;
+        for (const std::string &n : names) {
+            Digest dg;
+            const bool named = n.size() >= 64 && n.compare(0, 2, aa) == 0 && digest_from_hex(n.substr(0, 64).c_str(), dg.b) &&
+                               hex_of(dg.b, 32) == n.substr(0, 64);
+            struct stat st;
+            if (stat((dir + n).c_str(), &st) != 0 || !S_ISREG(st.st_mode)) continue;
+            const std::string tail = named ? n.substr(64) : n;
+            if (named && tail.empty()) {
+                auto &t = T.blobs[dg];
+                t.bytes += (uint64_t)st.st_size;
+                t.linked = st.st_nlink > 1;
+                ranked.push_back({stamp_of(st), TierKey{dg, false}});
+            } else if (named && tail == ".meta") {
+                metas[dg] = (uint64_t)st.st_size;
+            } else if (named && tail == ".part") {
+                if (!T.spills.count(dg)) unlink((dir + n).c_str());       // (a running spill's file is counted when placed)
+            } else {
+                T.blob_bytes += (uint64_t)st.st_size;     // not ours to remove; counted so the total is the tier's
+            }
+        }
+        for (auto &kv : metas) {
+            auto it = T.blobs.find(kv.first);
+            if (it != T.blobs.end()) it->second.bytes += kv.second;
+            else unlink((dir + hex_of(kv.first.b, 32) + ".meta").c_str());
+        }
+    }
+    for (auto &kv : T.blobs) T.blob_bytes += kv.second.bytes;
+    if (DIR *d = opendir((e->cas_dir + "/partial").c_str())) {
+        std::vector<std::string> names;
+        while (struct dirent *de = readdir(d)) if (de->d_name[0] != '.') names.emplace_back(de->d_name);
+        closedir(d);
+        for (const std::string &n : names) {
+            struct stat st;
+            if (stat((e->cas_dir + "/partial/" + n).c_str(), &st) != 0 || !S_ISREG(st.st_mode)) continue;
+            Digest dg;
+            const bool rec = n.size() == 69 && (n.compare(64, 5, ".ckpt") == 0 || n.compare(64, 5, ".part") == 0) &&
+                             digest_from_hex(n.substr(0, 64).c_str(), dg.b);
+            if (!rec) { T.partial_bytes += (uint64_t)st.st_size; continue; }
+            auto ins = T.saved.emplace(dg, TierEntry{});
+            ins.first->second.bytes += (uint64_t)st.st_size;
+            T.partial_bytes += (uint64_t)st.st_size;
+            if (ins.second) ranked.push_back({stamp_of(st), TierKey{dg, true}});
+        }
+    }
+    const std::string inc = e->cas_dir + "/incoming";
+    sweep_incoming(inc);
+    if (DIR *d = opendir(inc.c_str())) {
+        std::vector<std::string> names;
+        while (struct dirent *de = readdir(d)) if (de->d_name[0] != '.') names.emplace_back(de->d_name);
+        closedir(d);
+        for (const std::string &n : names) {
+            const uint64_t sz = file_size(inc + "/" + n);
+            tier_charge(T, T.staging[inc + "/" + n], 0, sz);
+        }
+    }
+    std::stable_sort(ranked.begin(), ranked.end(), [](const auto &a, const auto &b) { return a.first < b.first; });
+    for (auto &r : ranked) {
+        TierEntry &t = (r.second.saved ? T.saved : T.blobs)[r.second.d];
+        t.seq = ++T.seq;
+        T.order.emplace(t.seq, r.second);
+        T.last_stamp = std::max(T.last_stamp, r.first);
+    }
+    T.on = true;
+}
+
 bool spill_one(dm_engine *e, Blob *b)
 {
     const std::string path = blob_path(e, b->digest.b), tmp = path + ".part";
@@ -1181,19 +1541,25 @@ void spill_main(dm_engine *e)
             b = e->spill_q.front();
             e->spill_q.pop_front();
         }
+        tier_pin(e, b->digest, false, true);   // a running spill: its .part is not a leftover, its digest not a victim
         bool have;
+        std::string side;
         {
             std::lock_guard<std::mutex> g(e->mu);
             have = b->in_hbm;
-            if (have) b->readers++;        // pin against eviction while copying out
+            if (have) { b->readers++; side = sidecar_json(*b); }   // pin against eviction while copying out
         }
-        bool ok = have && spill_one(e, b.get());
+        TierRes res;
+        bool ok = have && tier_reserve(e, b->size + side.size(), false, &res) && spill_one(e, b.get());
+        if (ok) tier_placed(e, b->digest, false, &res, true);
+        else tier_release(e, res);
         {
             std::lock_guard<std::mutex> g(e->mu);
             if (have) b->readers--;
-            b->on_disk = ok;
+            b->on_disk = b->on_disk || ok;     // (a disk-backed publish or an import may have placed a copy meanwhile)
             b->spill_done = true;
         }
+        tier_unpin(e, b->digest, false, true);
         {
             std::lock_guard<std::mutex> g(e->spill_mu);
         }
@@ -1305,6 +1671,7 @@ static void disk_task_write(dm_engine *e, DiskTask &t)
     Stream *s = t.sp.get();
     const int err = pwrite_all(t.fd, t.slab->host, t.n, t.off);
     slab_return(e, t.slab);
+    if (!err) tier_stage_grow(e, s->path, t.off + t.n);     // (the path is stable while a write is in flight)
     {
         std::lock_guard<std::mutex> g(s->mu);
         if (err && s->lost == DM_OK) s->lost = fail(DM_EIO, "write to the disk-backed stream's file failed");
@@ -1374,31 +1741,40 @@ static void disk_task_publish(dm_engine *e, DiskTask &t)
     bool ok = keep && ftruncate(fd, (off_t)size) == 0 && (!(e->cfg.flags & DM_F_DISK_SYNC) || fsync(fd) == 0);
     if (fd >= 0) close(fd);
     std::shared_ptr<Blob> pub;
+    bool refused = false;                       // no room under the disk-tier limit: verified, not cached
     if (ok) {
         const std::string dst = blob_path(e, b->digest.b);
         mkdirs(dst);
+        tier_pin(e, b->digest);                 // not a victim while it is placed
+        TierRes res;
         struct stat st;
         const bool had = stat(dst.c_str(), &st) == 0;          // already in the disk tier: keep that copy
-        if (had) unlink(path.c_str());
+        if (had) { unlink(path.c_str()); tier_unstage(e, path); tier_touch(e, b->digest); }
+        else if (!tier_stage_to_blob(e, path, size, sidecar_json(*b).size(), &res)) refused = true;
         else ok = rename(path.c_str(), dst.c_str()) == 0;
-        if (ok && !had) write_sidecar(dst + ".meta", *b);
-    }
-    if (ok) {
-        std::lock_guard<std::mutex> gi(e->mu);
-        auto it = e->blobs.find(b->digest);
-        if (it != e->blobs.end()) pub = it->second;
-        else {
-            b->on_disk = b->spill_done = true;
-            e->blobs[b->digest] = b;
-            pub = b;
+        if (ok && !had && !refused) {
+            write_sidecar(dst + ".meta", *b);
+            tier_placed(e, b->digest, false, &res, true);
+        } else tier_release(e, res);
+        if (refused) ok = false;
+        if (ok) {                               // still pinned: the file the index now names cannot be evicted first
+            std::lock_guard<std::mutex> gi(e->mu);
+            auto it = e->blobs.find(b->digest);
+            if (it != e->blobs.end()) pub = it->second;
+            else {
+                b->on_disk = b->spill_done = true;
+                e->blobs[b->digest] = b;
+                pub = b;
+            }
+            if (!pub->on_disk) { pub->on_disk = true; pub->spill_done = true; }
         }
-        if (!pub->on_disk) { pub->on_disk = true; pub->spill_done = true; }
+        tier_unpin(e, b->digest);
     }
-    if (!ok) unlink(path.c_str());
+    if (!ok) { unlink(path.c_str()); tier_unstage(e, path); }
     if (ok) e->st_committed++;
-    else if (counted_mismatch || keep) e->st_mismatch++;
+    else if (counted_mismatch || (keep && !refused)) e->st_mismatch++;
     g.lock();
-    if (keep && !ok) { s->matched = 0; if (s->lost == DM_OK) s->lost = fail(DM_EIO, "could not move the verified file into the disk tier"); }
+    if (keep && !ok && !refused) { s->matched = 0; if (s->lost == DM_OK) s->lost = fail(DM_EIO, "could not move the verified file into the disk tier"); }
     s->publishing = false;
     s->blob = pub;
     if (s->st != St::Aborted) s->st = St::Done;

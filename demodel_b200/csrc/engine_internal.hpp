@@ -230,6 +230,7 @@ struct Reader {
     std::string disk_meta;        // sidecar text, disk-tier readers
     std::shared_ptr<Stream> follow;   // in-flight body this reader is coalesced onto (until it completes)
     int fd = -1;                  // disk tier
+    Digest disk_digest{};         // ... the blob it reads (pinned against disk-tier eviction while fd is open)
     uint64_t size = 0;
     std::mutex mu;                // a reader is normally one goroutine; this keeps misuse safe
     Window win[2];                // double-buffered read-ahead in pinned memory (HBM tier)
@@ -276,6 +277,35 @@ struct DiskTask {
     int fd = -1;
     uint64_t off = 0;
     uint32_t n = 0;
+};
+
+// The disk tier under a size limit (dm_cache_set_disk_limit).  Built by the first call with a non-zero limit (one walk
+// of blobs/, incoming/ and partial/) and dropped again by a limit of 0.  Every entry is a blob (file + sidecar) or a
+// saved download (.ckpt + .part); `order` ranks them least recently used first.  On disk the last use is the blob
+// file's mtime, written explicitly (content-addressed files are never rewritten, and reads never move it), except for
+// files with more than one link, whose recency lives in memory only.  Bytes are apparent sizes (st_size).
+struct TierEntry {
+    uint64_t bytes = 0;
+    uint64_t seq = 0;                     // key in DiskTier::order
+    bool linked = false;                  // st_nlink > 1 (a hard-linked import): its mtime is the source's, not ours
+};
+struct TierKey { Digest d; bool saved; };
+// Bytes set aside for a file that is about to be written (a spill, a saved download).  `gen` says which index they
+// were counted in: a reservation taken before the index was dropped and rebuilt is not returned to the new one.
+struct TierRes { uint64_t bytes = 0, gen = 0; bool partial = false; };
+struct DiskTier {
+    bool on = false;                      // a limit is set and the index below is built
+    uint64_t limit = 0, gen = 0, seq = 0;
+    int64_t last_stamp = 0;               // mtimes written are strictly increasing, so the order survives a restart
+    std::unordered_map<Digest, TierEntry, DigestHash> blobs, saved;
+    std::map<uint64_t, TierKey> order;
+    uint64_t blob_bytes = 0, partial_bytes = 0, staging_bytes = 0, reserved_blob = 0, reserved_partial = 0;
+    std::unordered_map<std::string, std::pair<uint64_t, uint64_t>> staging;   // incoming/ file -> (reserved, written)
+    // Pins: kept with or without a limit, so that a limit set later sees them.  Never evicted while counted.
+    std::unordered_map<Digest, uint32_t, DigestHash> pins, saved_pins;
+    std::unordered_map<Digest, uint32_t, DigestHash> spills;   // digests a spill is writing (<hex>.part under blobs/)
+    uint64_t evicted_files = 0, evicted_bytes = 0, refused = 0;
+    uint64_t used() const { return blob_bytes + reserved_blob + staging_bytes + partial_bytes + reserved_partial; }
 };
 
 }  // namespace dmi
@@ -405,6 +435,12 @@ struct dm_engine {
     FILE *alias_log = nullptr;
     std::atomic<uint64_t> n_suspended{0};   // *.ckpt under <cas_dir>/partial
 
+    // Disk-tier limit (struct DiskTier).  Lock order: tier_mu before e->mu (eviction updates the index under it), and
+    // never taken while e->mu is held.  A stream mutex may be held when it is taken; tier_mu never takes one.
+    std::mutex tier_mu;
+    DiskTier tier;
+    std::atomic<bool> tier_on{false};       // tier.on, readable without the lock: with no limit the hooks return at once
+
     std::mutex err_mu;               // dm_error_detail(): last error text by stream / reader id (bounded)
     std::unordered_map<uint64_t, std::string> err_text;
     std::deque<uint64_t> err_order;
@@ -499,5 +535,28 @@ int ensure_ingest_scratch(dm_engine *e, uint32_t n);
 void alias_load(dm_engine *e);                // dm_engine_create: replay <cas_dir>/aliases.log
 bool digest_from_hex(const char *hex, uint8_t out[32]);
 bool alias_key_ok(const char *key);           // 1..4096 bytes without control characters: one line of aliases.log
+void sweep_incoming(const std::string &dir);  // remove files under incoming/ of processes that are gone
+
+// Disk-tier limit (engine_core.cu).  None takes a stream mutex or may be called with e->mu held.  With no limit set
+// they only count pins; reservations always succeed and nothing is stat'ed, touched or written.
+void tier_pin(dm_engine *e, const Digest &d, bool saved = false, bool spill = false);   // spill: a running spill's pin
+void tier_unpin(dm_engine *e, const Digest &d, bool saved = false, bool spill = false);
+bool tier_reserve(dm_engine *e, uint64_t bytes, bool partial, TierRes *r);   // false: no room could be made (refused)
+void tier_release(dm_engine *e, TierRes &r);
+// The file(s) of `d` are in place (blobs/ or, saved, partial/): release `r`, enter them at their st_size; `use`: as
+// the most recently used entry.
+void tier_placed(dm_engine *e, const Digest &d, bool saved, TierRes *r, bool use);
+void tier_touch(dm_engine *e, const Digest &d);   // a use of blob d (no-op for blobs not in the tier)
+void tier_forget(dm_engine *e, const Digest &d, bool saved = false);   // its files were removed: count what is left
+// A file under incoming/ that will hold `reserve` bytes, `counted` of which the tier already counts elsewhere (a saved
+// download being resumed, whose entry goes when the resume takes it over); false: refused.
+bool tier_stage(dm_engine *e, const std::string &path, uint64_t reserve, uint64_t counted = 0);
+void tier_stage_grow(dm_engine *e, const std::string &path, uint64_t written);   // never refuses, never evicts
+void tier_unstage(dm_engine *e, const std::string &path);
+// The staged file at `path` is about to become a blob of `size` bytes with a `side`-byte sidecar: false (refused) when no
+// room can be made and none was reserved for the body when it was staged.
+bool tier_stage_to_blob(dm_engine *e, const std::string &path, uint64_t size, uint64_t side, TierRes *r);
+void tier_build(dm_engine *e);                         // tier_mu held: the walk that builds the index
+bool tier_make_room(dm_engine *e, uint64_t need, bool partial);   // tier_mu held: evict until `need` more bytes fit
 
 }  // namespace dmi

@@ -298,6 +298,19 @@ class Engine:
         raw = bytes(digs)
         return [(status[i], raw[32 * i:32 * i + 32]) for i in range(n)]
 
+    def set_disk_limit(self, limit_bytes: int) -> None:
+        """dm_cache_set_disk_limit: keep the disk tier at or under `limit_bytes` (apparent sizes), evicting least
+        recently used blobs and saved downloads that nothing pins; 0 turns the limit off.  The first non-zero limit
+        walks the tier once to build its index."""
+        check(self._lib.dm_cache_set_disk_limit(self._h, limit_bytes), "dm_cache_set_disk_limit")
+
+    def disk_usage(self) -> dict:
+        """dm_cache_disk_usage: limit, bytes in use by kind, eviction and refusal counters."""
+        u = _lib.DmDiskUsage()
+        u.struct_size = C.sizeof(_lib.DmDiskUsage)
+        check(self._lib.dm_cache_disk_usage(self._h, C.byref(u)), "dm_cache_disk_usage")
+        return {name: getattr(u, name) for name, _ in _lib.DmDiskUsage._fields_ if name not in ("struct_size", "reserved")}
+
     # -- URL-keyed requests (the OnRequest hook is handed a URL) -----------------------
     def alias_put(self, key: str, digest: bytes) -> None:
         check(self._lib.dm_cache_alias_put(self._h, key.encode(), _digest_arg(digest)), "dm_cache_alias_put")

@@ -62,6 +62,9 @@ type Config struct {
 	CacheDir      string // "" = HBM tier only
 	DiskSync      bool
 	DiskDirect    bool // bodies too large for HBM (all bodies when HBM holds none) are cached on disk; needs CacheDir
+	// DiskLimitBytes bounds the whole pool's disk tier (0 = no limit); each GPU's engine gets an equal share, since
+	// dm_shard_of splits digests evenly.  Needs CacheDir; a value below the GPU count is refused (DM_EINVAL).
+	DiskLimitBytes uint64
 }
 
 // Pool owns one engine per GPU and routes blobs by digest prefix
@@ -77,6 +80,9 @@ func Open(cfg Config) (*Pool, error) {
 	n := int(C.dm_device_count())
 	if n <= 0 {
 		return nil, &Error{Code: int(C.DM_ENODEV), Detail: "no CUDA device"}
+	}
+	if cfg.DiskLimitBytes > 0 && cfg.DiskLimitBytes < uint64(n) {
+		return nil, &Error{Code: int(C.DM_EINVAL), Detail: "DiskLimitBytes is smaller than one byte per GPU"}
 	}
 	p := &Pool{}
 	for dev := 0; dev < n; dev++ {
@@ -105,8 +111,35 @@ func Open(cfg Config) (*Pool, error) {
 			return nil, err
 		}
 		p.engines = append(p.engines, e)
+		if cfg.DiskLimitBytes > 0 {
+			if err := check(e, 0, C.dm_cache_set_disk_limit(e, C.uint64_t(cfg.DiskLimitBytes/uint64(n)))); err != nil {
+				p.Close()
+				return nil, err
+			}
+		}
 	}
 	return p, nil
+}
+
+// DiskUsage mirrors dm_disk_usage for one GPU's engine.
+type DiskUsage struct {
+	LimitBytes, UsedBytes, BlobFiles, BlobBytes, StagingBytes, PartialBytes uint64
+	EvictedFiles, EvictedBytes, Refused                                      uint64
+}
+
+// DiskUsage reports each engine's disk tier, in GPU order.
+func (p *Pool) DiskUsage() []DiskUsage {
+	out := make([]DiskUsage, len(p.engines))
+	for i, e := range p.engines {
+		var u C.dm_disk_usage
+		u.struct_size = C.uint32_t(unsafe.Sizeof(u))
+		if C.dm_cache_disk_usage(e, &u) != C.DM_OK {
+			continue
+		}
+		out[i] = DiskUsage{uint64(u.limit_bytes), uint64(u.used_bytes), uint64(u.blob_files), uint64(u.blob_bytes),
+			uint64(u.staging_bytes), uint64(u.partial_bytes), uint64(u.evicted_files), uint64(u.evicted_bytes), uint64(u.refused)}
+	}
+	return out
 }
 
 func (p *Pool) Close() {

@@ -42,7 +42,8 @@ extern "C" {
 typedef enum dm_err {
     DM_OK        = 0,
     DM_EINVAL    = -1,   /* bad argument / unknown id */
-    DM_ENOMEM    = -2,   /* HBM arena, pinned ring or stream table exhausted */
+    DM_ENOMEM    = -2,   /* HBM arena, pinned ring or stream table exhausted; or no room under the disk-tier limit
+                          * (dm_cache_import, dm_stream_suspend: see dm_cache_set_disk_limit) */
     DM_ENOENT    = -3,   /* digest not in the content-addressed store */
     DM_ECUDA     = -4,   /* CUDA runtime error; dm_last_error() has the text */
     DM_ESTATE    = -5,   /* call not valid in the stream's current state */
@@ -307,7 +308,8 @@ int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, u
  *   DM_EINVAL    not a regular file
  *   DM_EIO       the source could not be read, or the copy could not be written, renamed or given its sidecar
  *   DM_ECUDA     a copy or launch failed
- *   DM_ENOMEM    no stream slot to spare (the budget of dm_cache_promote and dm_cache_verify, shared with them)
+ *   DM_ENOMEM    no stream slot to spare (the budget of dm_cache_promote and dm_cache_verify, shared with them), or
+ *                no room for it under the disk-tier limit (dm_cache_set_disk_limit)
  * After any of these the source is untouched, bytes and inode, and <cas_dir>/incoming/ holds nothing of the call.
  * Duplicate entries (same path and expect row) are imported once; each gets the status, digest and its own alias.
  * Threads, slot budget and ring share are dm_cache_verify's.  bytes_hashed and h2d_bytes grow by the bytes hashed,
@@ -318,6 +320,69 @@ int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, u
  * would refuse, an unknown flag); DM_ESTATE without cas_dir. */
 int dm_cache_import(dm_engine *e, const char *const *paths, const uint8_t *expect, const char *const *keys,
                     uint32_t n, uint32_t flags, uint8_t *digests_out, int32_t *status_out);
+/* Keep the disk tier under a size limit.  Opt-in: an engine that never sets one touches, scans and reserves nothing.
+ * Bytes are apparent sizes (st_size) of the regular files under <cas_dir>/blobs/, incoming/ and partial/
+ * (aliases.log is not counted).  A hard-linked import (DM_IMP_LINK) counts at its full size although its inode is
+ * shared with the source.  With a limit set, a cas_dir belongs to ONE engine (the Go pool gives each GPU <dir>/gpu<N>).
+ * The limit is not a free-space guard: other writers on the filesystem are not seen.
+ *
+ * dm_cache_set_disk_limit: limit_bytes = 0 turns the limit off again (the index is dropped).  The first call with a
+ * non-zero limit builds the disk index synchronously: one walk of blobs/, incoming/ and partial/ with one stat per name
+ * (the walk dm_cache_list does), which also removes spill leftovers (<hex>.part under blobs/ with no spill of this engine
+ * running), sidecars whose blob file is missing and incoming/ files of processes that are gone.  Every call then evicts
+ * until used_bytes <= limit_bytes or only pinned entries are left, and returns DM_OK either way (dm_cache_disk_usage
+ * shows which).  DM_ESTATE without cas_dir.  The walk and each eviction's unlinks run under the tier's lock, which
+ * disk-tier opens (dm_cache_open of a blob not in HBM) and spills also take for their pins, with or without a limit:
+ * they wait for the first walk (about 4 s per 100 000 files on tmpfs) and for the evictions of a placement.
+ *
+ * Recency.  Entries - blobs (file + sidecar) and saved downloads (.ckpt + .part) - are evicted least recently used
+ * first.  A use is a placement (spill, disk-backed publish, import), dm_cache_open served from disk, dm_cache_promote
+ * returning DM_OK, and a blob leaving HBM.  dm_cache_verify, dm_cache_list, dm_cache_contains and an import that finds
+ * the digest already cached are not uses.  The last use is stored as the blob file's mtime (written explicitly; reads
+ * never move it), so the order survives a restart; files with more than one link keep their recency in memory only,
+ * since writing their mtime would modify an import's source.  HBM-resident blobs rank above every disk-only entry: their
+ * disk copies go only after every evictable disk-only entry, in HBM LRU order, and such a blob stays servable from HBM
+ * and is dropped when it leaves HBM (it is not written to disk again).
+ *
+ * Room.  Each placement reserves its bytes before they reach the disk, evicting as needed.  When no room can be made:
+ *   spill of an HBM blob (size + sidecar)     skipped, as after a failed spill (DM_F_DISK_SYNC finish: DM_EIO); refused++
+ *   disk-backed stream with size_hint         opens verify-only: verified, not cached, no file in incoming/; refused++.
+ *                                             Once open its room is kept: it is placed at publish even if unknown-size
+ *                                             bodies have run the tier over the limit meanwhile (not if the limit has
+ *                                             been lowered below its size)
+ *   disk-backed stream of unknown size        never failed by the limit: charged as it is written and may run over the
+ *                                             limit while live (the overshoot is bounded by the unknown-size disk-backed
+ *                                             bodies in flight).  At publish its final size must fit: if not, the file is
+ *                                             removed, dm_stream_finish returns DM_OK with *matched as the digest says,
+ *                                             nothing is cached; refused++
+ *   dm_cache_import staging copy (its size)   DM_ENOMEM for that entry: the source is untouched, nothing in incoming/
+ *   dm_stream_suspend of an HBM stream        DM_ENOMEM, the stream stays open
+ *   suspend / resume of a disk-backed stream  nothing new: its bytes move between incoming/ and partial/ (a resumed
+ *                                             stream makes room for its size_hint less the bytes saved)
+ *
+ * Pins: never evicted while a disk reader has the blob open (until dm_cache_close), while a dm_cache_promote,
+ * dm_cache_verify or dm_cache_import call holds the digest, while a disk-backed stream publishes it or a spill writes
+ * it, and while dm_stream_resume_saved takes a saved download over.  Evicting a blob removes its file, then its sidecar;
+ * its aliases stay (dm_cache_open then misses).  Evicting a saved download removes .ckpt, then .part; a later
+ * dm_stream_resume_saved for it is DM_ENOENT.  A reader that opened a file just before its eviction keeps reading its
+ * descriptor. */
+typedef struct dm_disk_usage {
+    uint32_t struct_size;      /* = sizeof(dm_disk_usage); ABI guard */
+    uint32_t reserved;
+    uint64_t limit_bytes;      /* 0 = no limit (the default) */
+    uint64_t used_bytes;       /* blob_bytes + staging_bytes + partial_bytes */
+    uint64_t blob_files;       /* blobs in blobs/sha256/ */
+    uint64_t blob_bytes;       /* their files + sidecars, plus spills being written (at their reservation) */
+    uint64_t staging_bytes;    /* incoming/: disk-backed streams and import copies, at max(reservation, written) */
+    uint64_t partial_bytes;    /* partial/: downloads saved by dm_stream_suspend (.ckpt + .part) */
+    uint64_t evicted_files;    /* blobs and saved downloads removed to stay under the limit, since create */
+    uint64_t evicted_bytes;
+    uint64_t refused;          /* placements skipped because no room could be made (see above) */
+} dm_disk_usage;
+int dm_cache_set_disk_limit(dm_engine *e, uint64_t limit_bytes);
+/* DM_EINVAL on a wrong struct_size.  Without a limit set: limit_bytes = 0, the three counters, zero for the rest (it
+ * never walks the directory by itself). */
+int dm_cache_disk_usage(dm_engine *e, dm_disk_usage *out);
 /* Request coalescing: the blob is not cached yet but another connection is
  * ingesting it right now (a stream opened with this expected digest).  The
  * reader follows that body out of HBM: dm_cache_read blocks until bytes past
