@@ -460,7 +460,8 @@ static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t siz
         e->streams[k][sp->id] = sp;
         e->n_streams++;
     }
-    if (followable && sp->has_expect && !sp->verify_only) {          // first opener wins; later duplicates are not followable
+    // followable: a stream that keeps its bytes, in HBM or in its file (a verify-only stream retains nothing to serve)
+    if (followable && sp->has_expect && (!sp->verify_only || sp->disk)) {   // first opener wins; later duplicates are not followable
         std::lock_guard<std::mutex> g(e->mu);
         auto &slot = e->inflight[sp->expect];
         if (slot.expired()) slot = sp;
@@ -662,7 +663,8 @@ static int stream_resume_impl(dm_engine *e, const dm_checkpoint *ck, const uint8
     Stream *s = sp.get();
     std::unique_lock<std::mutex> g(s->mu);
     s->resume_base = s->dma_issued = s->hash_issued = s->landed = s->staged_to = ck->bytes;
-    if (ck->bytes == 0 && s->has_expect && !s->verify_only) {
+    // (a disk-backed stream taking over a saved file is registered by dm_stream_resume_saved once the file holds [0, C))
+    if (ck->bytes == 0 && s->has_expect && (!s->verify_only || (s->disk && saved == 0))) {
         std::lock_guard<std::mutex> g2(e->mu);
         auto &slot = e->inflight[s->expect];
         if (slot.expired()) slot = sp;
@@ -771,6 +773,8 @@ static int suspend_disk(dm_engine *e, const std::shared_ptr<Stream> &sp, uint64_
     struct stat st;
     const bool fresh = stat((base + ".ckpt").c_str(), &st) != 0;
     unlink((base + ".ckpt").c_str());                    // an older record must not pair with the new bytes
+    { std::lock_guard<std::mutex> g(s->mu); s->cuts++; }     // followers: what they read past C from now on is not the body's
+    s->cv.notify_all();
     bool ok = ftruncate(fd, (off_t)saved) == 0 && rename(path.c_str(), (base + ".part").c_str()) == 0;
     const bool moved = ok;
     FILE *f = ok ? fopen((base + ".ckpt.tmp").c_str(), "wb") : nullptr;
@@ -990,6 +994,17 @@ static int resume_saved_pinned(dm_engine *e, const uint8_t expect[32], uint64_t 
     unlink((base + ".part").c_str());
     if (e->n_suspended) e->n_suspended--;
     tier_forget(e, dg, true);
+    if (auto sp = find_stream(e, *id)) {
+        // a disk-backed stream's file holds the saved bytes from byte 0 now (adopted, or written back above as they
+        // land): followable from byte 0, first opener wins
+        bool disk;
+        { std::lock_guard<std::mutex> g(sp->mu); disk = sp->disk && sp->fd >= 0 && sp->st == St::Open; }
+        if (disk) {
+            std::lock_guard<std::mutex> g(e->mu);
+            auto &slot = e->inflight[sp->expect];
+            if (slot.expired()) slot = sp;
+        }
+    }
     if (resume_from) *resume_from = saved;
     return DM_OK;
 }

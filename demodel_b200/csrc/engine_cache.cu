@@ -47,6 +47,7 @@ static int cache_open_impl(dm_engine *e, const uint8_t digest[32], uint64_t *rea
         r->fd = open(blob_path(e, digest).c_str(), O_RDONLY);
         if (r->fd < 0) { tier_unpin(e, d); return DM_ENOENT; }
         r->disk_digest = d;
+        r->disk_pin = true;
         tier_touch(e, d);
         struct stat st;
         fstat(r->fd, &st);
@@ -75,6 +76,68 @@ static std::shared_ptr<Reader> find_reader(dm_engine *e, uint64_t id)
     return it == e->readers[id % kStripes].end() ? nullptr : it->second;
 }
 
+// follow_read of a disk-backed body: the reader has its own descriptor of the body's file and serves bytes whose pwrite
+// has completed (Stream::written), pread straight into the caller's buffer.  It holds no stream lock during the pread
+// and nothing the stream waits for: the descriptor keeps the inode alive through an abort's unlink, and a publication's
+// rename makes that inode the tier file.  Written bytes are never rewritten; only a suspend's cut removes some, so a
+// read that overlaps a cut (Stream::cuts moved) fails rather than return what the file holds now.  Reader mutex held.
+static int follow_disk_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t len, size_t *nread)
+{
+    Stream *s = r->follow.get();
+    uint64_t end = 0;                           // end of the written range holding `off`
+    {
+        std::unique_lock<std::mutex> g(s->mu);
+        auto avail = [&] {
+            auto it = s->written.upper_bound(off);
+            end = it != s->written.begin() && std::prev(it)->second > off ? std::prev(it)->second : 0;
+            return end > off;
+        };
+        s->followers++;
+        s->cv.wait(g, [&] {
+            return s->cuts != r->follow_cut || s->st == St::Done || s->st == St::Aborted || s->lost != DM_OK || len == 0 ||
+                   avail();
+        });
+        s->followers--;
+        if (s->cuts != r->follow_cut)
+            return fail(DM_ESTATE, "the body this reader followed was suspended (dm_stream_suspend): follow it again once it is resumed");
+        if (s->st == St::Aborted) return fail(DM_ESTATE, "the upstream body this reader followed was aborted");
+        if (s->lost != DM_OK) return fail(DM_ESTATE, "a write to the file of the body this reader followed failed (DM_EIO): nothing of it is cached");
+        if (s->st == St::Done) {
+            if (s->cuda_failed) return fail(DM_ESTATE, "a CUDA copy or launch failed while the body this reader followed was hashed");
+            if (!s->matched) return fail(DM_ESTATE, "the upstream body this reader followed failed verification");
+            // verified: from now on an ordinary disk-tier reader of its descriptor, whose inode is the tier file if the
+            // body was placed there (pinned like dm_cache_open's), else a file only this reader still has open
+            const bool placed = s->blob != nullptr;
+            r->size = s->dma_issued;
+            r->disk_meta = s->sidecar;
+            r->disk_digest = s->digest;
+            g.unlock();
+            if (placed) { tier_pin(e, r->disk_digest); r->disk_pin = true; }
+            r->follow.reset();
+            return 1;
+        }
+        if (len == 0) return DM_OK;
+    }
+    const size_t n = (size_t)std::min<uint64_t>(len, end - off);
+    uint8_t *out = static_cast<uint8_t *>(buf);
+    size_t got = 0;
+    while (got < n) {
+        const ssize_t k = pread(r->fd, out + got, n - got, (off_t)(off + got));
+        if (k < 0 && errno == EINTR) continue;
+        if (k <= 0) break;
+        got += (size_t)k;
+    }
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        if (s->cuts != r->follow_cut)
+            return fail(DM_ESTATE, "the body this reader followed was suspended (dm_stream_suspend): follow it again once it is resumed");
+        if (got < n) return fail(DM_ESTATE, "the file of the body this reader followed could not be read");
+    }
+    e->st_served += got;
+    if (nread) *nread = got;
+    return DM_OK;
+}
+
 // Read from a body that is still arriving (request coalescing).  Blocks until bytes past `off` have
 // been DMA'd, the body completes, or it fails.  Returns DM_OK with *nread set, a dm_err, or 1 when the
 // body has completed and been published (the reader has been switched to the blob; caller continues).
@@ -83,6 +146,7 @@ static int follow_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t 
     std::lock_guard<std::mutex> gr(r->mu);
     if (!r->follow) return 1;
     Stream *s = r->follow.get();
+    if (s->disk) return follow_disk_read(e, r, off, buf, len, nread);
     std::vector<std::pair<uint8_t *, uint64_t>> segs;
     size_t n = 0;
     {
@@ -298,7 +362,10 @@ static int cache_close_impl(dm_engine *e, uint64_t reader)
         std::lock_guard<std::mutex> g(e->mu);
         r->blob->readers--;
     }
-    if (r->fd >= 0) { close(r->fd); tier_unpin(e, r->disk_digest); }
+    if (r->fd >= 0) {
+        close(r->fd);
+        if (r->disk_pin) tier_unpin(e, r->disk_digest);
+    }
     return DM_OK;
 }
 
@@ -316,6 +383,20 @@ static int cache_follow_impl(dm_engine *e, const uint8_t digest[32], uint64_t *r
         r->follow = it->second.lock();
         if (!r->follow) { e->inflight.erase(it); return DM_ENOENT; }
         id = e->next_id.fetch_add(1);
+    }
+    if (Stream *s = r->follow.get(); s->disk) {
+        // the follower's own descriptor, taken before the stream can close its own (publication, abort, suspend)
+        std::unique_lock<std::mutex> g(s->mu);
+        if (s->fd < 0) {
+            if (s->st == St::Aborted || s->lost != DM_OK) return DM_ENOENT;
+            s->cv.wait(g, [&] { return !s->publishing; });         // being renamed into the tier: a hit in a moment
+            g.unlock();
+            return cache_open_impl(e, digest, reader, size_hint);
+        }
+        if (s->st == St::Aborted || s->lost != DM_OK || s->suspending) return DM_ENOENT;
+        r->fd = fcntl(s->fd, F_DUPFD_CLOEXEC, 0);
+        if (r->fd < 0) return fail(DM_EIO, "could not duplicate the descriptor of the followed body's file");
+        r->follow_cut = s->cuts;
     }
     r->size = r->follow->size_hint;
     {

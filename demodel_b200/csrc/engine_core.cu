@@ -1738,6 +1738,7 @@ static void disk_task_publish(dm_engine *e, DiskTask &t)
     b->meta.swap(s->meta);
     const bool counted_mismatch = !s->matched;
     g.unlock();
+    std::string side = sidecar_json(*b);
     bool ok = keep && ftruncate(fd, (off_t)size) == 0 && (!(e->cfg.flags & DM_F_DISK_SYNC) || fsync(fd) == 0);
     if (fd >= 0) close(fd);
     std::shared_ptr<Blob> pub;
@@ -1750,7 +1751,7 @@ static void disk_task_publish(dm_engine *e, DiskTask &t)
         struct stat st;
         const bool had = stat(dst.c_str(), &st) == 0;          // already in the disk tier: keep that copy
         if (had) { unlink(path.c_str()); tier_unstage(e, path); tier_touch(e, b->digest); }
-        else if (!tier_stage_to_blob(e, path, size, sidecar_json(*b).size(), &res)) refused = true;
+        else if (!tier_stage_to_blob(e, path, size, side.size(), &res)) refused = true;
         else ok = rename(path.c_str(), dst.c_str()) == 0;
         if (ok && !had && !refused) {
             write_sidecar(dst + ".meta", *b);
@@ -1777,6 +1778,7 @@ static void disk_task_publish(dm_engine *e, DiskTask &t)
     if (keep && !ok && !refused) { s->matched = 0; if (s->lost == DM_OK) s->lost = fail(DM_EIO, "could not move the verified file into the disk tier"); }
     s->publishing = false;
     s->blob = pub;
+    s->sidecar.swap(side);
     if (s->st != St::Aborted) s->st = St::Done;
     g.unlock();
     s->cv.notify_all();

@@ -192,6 +192,8 @@ struct Stream {
     uint32_t disk_writes = 0, disk_reads = 0;    // in flight on the disk threads (at most one read)
     bool publishing = false;                     // the final rename / sidecar is running on a disk thread
     bool suspending = false;                     // dm_stream_suspend: no further read-back or launch
+    uint32_t cuts = 0;                           // dm_stream_suspend cut the file at C: followers' bytes past C are gone
+    std::string sidecar;                         // the sidecar text of the verified body (followers' dm_cache_meta)
     // dm_cache_verify / dm_cache_import: a check of a stored file, never a download.  A disk-backed check reads the
     // file itself (fd / path, every byte already written: a blob file, or an import's staged copy); a tiny one travels
     // in a pack as a hash-only member.  It holds no arena extent, and its verdict is all it produces: nothing is
@@ -229,8 +231,10 @@ struct Reader {
     std::shared_ptr<Blob> blob;
     std::string disk_meta;        // sidecar text, disk-tier readers
     std::shared_ptr<Stream> follow;   // in-flight body this reader is coalesced onto (until it completes)
-    int fd = -1;                  // disk tier
-    Digest disk_digest{};         // ... the blob it reads (pinned against disk-tier eviction while fd is open)
+    int fd = -1;                  // disk tier; a follower of a disk-backed body: its own descriptor of the body's file
+    Digest disk_digest{};         // ... the blob it reads
+    bool disk_pin = false;        // ... pinned against disk-tier eviction until dm_cache_close
+    uint32_t follow_cut = 0;      // Stream::cuts when a disk-backed body was followed
     uint64_t size = 0;
     std::mutex mu;                // a reader is normally one goroutine; this keeps misuse safe
     Window win[2];                // double-buffered read-ahead in pinned memory (HBM tier)

@@ -200,7 +200,11 @@ class Engine:
         return rid.value, size.value
 
     def cache_follow(self, digest: bytes) -> Optional[tuple[int, int]]:
-        """Attach to a body that is still being ingested (request coalescing): (reader, size_hint) or None."""
+        """Attach to a body that is still being ingested (request coalescing): (reader, size_hint) or None.
+
+        size_hint is 0 when the body's size is unknown.  Reads block until the bytes have arrived: in HBM, or, for a
+        disk-backed body (DM_F_DISK_DIRECT), in its file; the read at EOF waits for the verdict.  A failed, aborted or
+        suspended body makes reads raise DM_ESTATE.  None also for a stream that retains nothing to serve."""
         rid, size = C.c_uint64(), C.c_uint64()
         rc = self._lib.dm_cache_follow(self._h, _digest_arg(digest), C.byref(rid), C.byref(size))
         if rc == DM_ENOENT:

@@ -430,7 +430,13 @@ func (r *HitReader) Meta() (string, error) {
 }
 
 // Follow attaches to a body another connection is ingesting right now
-// (request coalescing); nil if nothing is in flight for this digest.
+// (request coalescing); nil if nothing is in flight for this digest, or if the
+// stream retains nothing to serve (verify-only).  Reads block until the bytes
+// have arrived - in HBM, or in the file of a disk-backed body (DM_F_DISK_DIRECT),
+// served as its writes complete - and the read at EOF waits for the verdict,
+// which for a disk-backed body means until the GPU has hashed the whole file.
+// An aborted, corrupt or suspended body makes Read return an *Error with
+// DM_ESTATE; after a suspend, Follow again once the download is resumed.
 func (p *Pool) Follow(digest *[32]byte) *HitReader {
 	e := p.engineFor(digest)
 	var id, size C.uint64_t

@@ -68,7 +68,8 @@ typedef struct dm_engine dm_engine;   /* opaque; owned by caller between create/
                                   * instead: its bytes are written to <cas_dir>/incoming/ as they arrive, each ring slab
                                   * returns as soon as its write completes, the GPU hashes the bytes read back from that
                                   * file, and the verified file is renamed into the disk tier.  Range parts, suspend and
-                                  * resume work as on HBM streams; followers (dm_cache_follow) do not attach to them. */
+                                  * resume work as on HBM streams, and followers (dm_cache_follow) attach to them: they
+                                  * read the body from its file as its writes complete (see dm_cache_follow). */
 
 typedef struct dm_config {
     uint32_t struct_size;     /* = sizeof(dm_config); ABI guard */
@@ -365,7 +366,7 @@ int dm_cache_import(dm_engine *e, const char *const *paths, const uint8_t *expec
  * it, and while dm_stream_resume_saved takes a saved download over.  Evicting a blob removes its file, then its sidecar;
  * its aliases stay (dm_cache_open then misses).  Evicting a saved download removes .ckpt, then .part; a later
  * dm_stream_resume_saved for it is DM_ENOENT.  A reader that opened a file just before its eviction keeps reading its
- * descriptor. */
+ * descriptor.  A follower of a disk-backed body (dm_cache_follow) pins the blob as a disk reader from its EOF read on. */
 typedef struct dm_disk_usage {
     uint32_t struct_size;      /* = sizeof(dm_disk_usage); ABI guard */
     uint32_t reserved;
@@ -384,12 +385,38 @@ int dm_cache_set_disk_limit(dm_engine *e, uint64_t limit_bytes);
  * never walks the directory by itself). */
 int dm_cache_disk_usage(dm_engine *e, dm_disk_usage *out);
 /* Request coalescing: the blob is not cached yet but another connection is
- * ingesting it right now (a stream opened with this expected digest).  The
- * reader follows that body out of HBM: dm_cache_read blocks until bytes past
- * `off` have arrived, and once the body completes and verifies the reader
- * becomes an ordinary cache reader.  If the body is aborted or fails
- * verification, reads fail with DM_ESTATE.  DM_ENOENT: nothing in flight.
- * *size_hint = the Content-Length the ingesting stream was opened with (0 = unknown). */
+ * ingesting it right now (a stream opened with this expected digest; the first
+ * one opened is followed).  The reader follows that body out of HBM:
+ * dm_cache_read blocks until bytes past `off` have arrived, and once the body
+ * completes and verifies the reader becomes an ordinary cache reader.  If the
+ * body is aborted or fails verification, reads fail with DM_ESTATE.
+ * DM_ENOENT: nothing in flight, or a stream that retains nothing to serve (a
+ * verify-only stream: DM_F_NO_HBM_CAS or over-arena without DM_F_DISK_DIRECT,
+ * or a disk-backed open the disk-tier limit refused).
+ * *size_hint = the Content-Length the ingesting stream was opened with (0 = unknown).
+ * A body the GPU hashes once is read by any number of followers.
+ *
+ * Disk-backed bodies (DM_F_DISK_DIRECT), from dm_stream_open on, and from byte 0 again once dm_stream_resume_saved
+ * has taken a saved download over (its file holds the saved prefix):
+ *   - the follower keeps a descriptor of the body's file of its own (a body whose file is being renamed into the tier
+ *     at that moment is opened as dm_cache_open opens it), and dm_cache_read blocks until `off` lies in a
+ *     range whose file write has completed, then reads from the file straight into buf, up to the end of that range.
+ *     Range parts are served as they land: a reader inside a later part does not wait for the prefix.
+ *   - the read at EOF (off = the size, known or final) returns once the verdict is in: after the GPU has hashed the
+ *     whole file, which for one body runs at one hash chain's rate (tens of MB/s).  Verified, the reader is an
+ *     ordinary disk-tier reader of its descriptor: dm_cache_meta returns the published sidecar and, when the blob was
+ *     placed in the tier, the blob is pinned against disk-tier eviction until dm_cache_close, as a dm_cache_open
+ *     reader's is.  A verified body that was not placed (no room under the limit, or the tier already had it) is still
+ *     read to the end from the descriptor.
+ *   - an abort, a mismatch, a failed file write (DM_EIO), a failed copy or launch and dm_stream_suspend wake blocked
+ *     followers; their reads return DM_ESTATE, and dm_error_detail(reader) says which it was.  A read that would
+ *     return bytes past a suspend's cut returns DM_ESTATE too, never short data.  Follow again after
+ *     dm_stream_resume_saved.
+ *   - nothing a follower holds delays an abort, a publication or a suspend.  Its descriptor of a file that is
+ *     unlinked or evicted later keeps the bytes readable and is not counted by the disk-tier limit, as an open disk
+ *     reader's is not.
+ *   - bytes_served grows by what followers read; bytes_hashed and h2d_bytes by the body once.  open_readers counts
+ *     followers. */
 int dm_cache_follow(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size_hint);
 
 /* URL -> digest index for the OnRequest hit check (start.go:197-200 hands the hook a request, not a
