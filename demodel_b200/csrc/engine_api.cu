@@ -145,6 +145,7 @@ void dm_engine_destroy(dm_engine *e)
 {
     if (!e) return;
     cudaSetDevice(e->device);
+    load_stop_all(e);                             // first: a loader may be waiting for ring slabs the pump gives back
     {
         std::lock_guard<std::mutex> g(e->work_mu);
         e->stop = true;
@@ -1186,25 +1187,27 @@ static int stream_abort_impl(dm_engine *e, uint64_t id)
     return DM_OK;
 }
 
-// ---- promotion: disk tier -> HBM (dm_cache_promote) ------------------------------------
+// ---- loads: disk tier -> HBM (dm_cache_promote, dm_cache_open_verified) -----------------
 // Each blob is an internal stream opened with expect = its digest and size_hint = its file size: the file is pread
 // into acquired ring windows, flushed, and the next file starts while the pump hashes it.  The blob is registered as
 // disk-only first, so publish() re-homes it into HBM without queueing a spill: the verified file keeps its inode.
+// A running load is in e->loads under its digest (struct Load): a second promotion or verified open of the digest waits
+// for it or reads along instead of loading the file again.
 
 namespace {
 
 constexpr int kPromoteThreads = 4;        // loaders: reads of different files overlap
+constexpr int kLoadThreads = 4;           // the engine's loader threads (dm_cache_open_verified)
 // Tiny bodies are flushed this many at a time.  Their hash takes less time than reading the next file, so one by one
 // each would be a launch of its own; together they share a pack DMA and a launch.
 constexpr size_t kPromoteTinyBatch = 256;
+const char *kCorruptText = "the disk tier file does not hash to its digest: file and sidecar removed";
 
 struct Promotion {
     Digest d;
     int32_t status = DM_ENOENT;
-    uint64_t stream = 0;                  // open: the verdict is still to be collected
-    bool tiny = false;                    // at most tiny_max bytes, written to the stream's private buffer, not flushed yet
-    struct stat seen{};                   // the file that was read (st_dev / st_ino)
-    std::shared_ptr<Blob> mine;           // the disk-only entry this promotion registered (none if one existed)
+    std::shared_ptr<Load> load;           // the load this promotion runs (own), or the running one it waits for
+    bool own = false;
 };
 
 // The sidecar's top-level "size" (it precedes "headers", so the first match is it).  The number must be followed by
@@ -1253,11 +1256,11 @@ void drop_corrupt(dm_engine *e, const Digest &d, const struct stat &seen)
     if (!exists || same) { tier_forget(e, d); forget_disk_copy(e, d, nullptr); }
 }
 
-// The promotion ended without a verdict on the file (no slot or room, a failed read, copy or launch): take back the
+// The load ended without a verdict on the file (no slot or room, a failed read, copy or launch): take back the
 // entry it registered, which carries the file's unverified size.
-void promote_undo(dm_engine *e, Promotion &p)
+void load_undo(dm_engine *e, Load &L)
 {
-    if (p.mine) forget_disk_copy(e, p.d, p.mine.get());
+    if (L.mine) forget_disk_copy(e, L.d, L.mine.get());
 }
 
 // Open the disk copy of `d` for a check: *fd open O_RDONLY, `seen` its fstat, `side` its sidecar text ("" if none).
@@ -1288,58 +1291,101 @@ int open_disk_copy(dm_engine *e, const Digest &d, int *fd, struct stat *seen, st
     return DM_OK;
 }
 
-// Start loading one blob.  Returns 1 with p.stream open (and flushed unless p.tiny), or the blob's final status.
-// `tiny_buf` holds tiny_max bytes: a tiny body is read there and written into its stream's private buffer, so that it
-// holds no ring slab while it waits for its batch's flush.  `may_open`: false when the call has no stream slot to spare.
-int promote_start(dm_engine *e, Promotion &p, uint8_t *tiny_buf, bool may_open)
+// Every outcome of a claimed load ends here: it leaves the index, and whoever waits for it (readers, promotions) wakes.
+void load_end(dm_engine *e, Load &L, int status, const char *why)
 {
     {
         std::lock_guard<std::mutex> g(e->mu);
-        auto it = e->blobs.find(p.d);
-        if (it != e->blobs.end() && it->second->in_hbm) return DM_OK;
+        auto it = e->loads.find(L.d);
+        if (it != e->loads.end() && it->second.get() == &L) e->loads.erase(it);
     }
-    int fd;
+    {
+        std::lock_guard<std::mutex> g(L.mu);
+        L.done = true;
+        L.status = status;
+        if (status != DM_OK) L.why = why;
+    }
+    L.cv.notify_all();
+}
+
+int load_wait(Load &L)
+{
+    std::unique_lock<std::mutex> g(L.mu);
+    L.cv.wait(g, [&] { return L.done; });
+    return L.status;
+}
+
+// Open the stream of a claimed load on the calling thread: the file and its sidecar, the size checks, the stream (its
+// HBM extent reserved, evicting LRU blobs) and the disk-only index entry.  Returns 1 with the stream open and L.fd left
+// open for load_fill, or the load's final status (L.fd closed): DM_OK when a stream published the blob meanwhile.
+// `may_open`: false when the call has no stream slot to spare.
+int load_open(dm_engine *e, Load &L, bool may_open)
+{
     std::string side;
-    if (int rc = open_disk_copy(e, p.d, &fd, &p.seen, &side); rc != DM_OK) return rc;
-    const uint64_t size = (uint64_t)p.seen.st_size;
+    if (int rc = open_disk_copy(e, L.d, &L.fd, &L.seen, &side); rc != DM_OK) return rc;
+    const uint64_t size = (uint64_t)L.seen.st_size;
+    auto shut = [&] { close(L.fd); L.fd = -1; };
     // checked here: a stream with this size_hint would silently become verify-only or disk-backed
-    if (size > e->cfg.hbm_cas_bytes) { close(fd); return fail(DM_ENOMEM, "blob is larger than the HBM arena"); }
-    if (!may_open) { close(fd); return fail(DM_ENOMEM, "no stream slot to spare for a promotion"); }
+    if (size > e->cfg.hbm_cas_bytes) { shut(); return fail(DM_ENOMEM, "blob is larger than the HBM arena"); }
+    if (!may_open) { shut(); return fail(DM_ENOMEM, "no stream slot to spare for a load of a disk tier blob"); }
     uint64_t id = 0;
-    int rc = stream_open_impl(e, p.d.b, size, &id, false);
-    if (rc != DM_OK) { close(fd); return rc; }
+    int rc = stream_open_impl(e, L.d.b, size, &id, false);
+    if (rc != DM_OK) { shut(); return rc; }
     bool in_hbm = false;                                 // a stream published it meanwhile
     {
         // registered before the verdict (publish() then re-homes it without a spill); taken back on every outcome
         // that does not verify the file
         std::lock_guard<std::mutex> g(e->mu);
-        auto it = e->blobs.find(p.d);
+        auto it = e->blobs.find(L.d);
         if (it != e->blobs.end() && it->second->in_hbm) in_hbm = true;
         else if (it == e->blobs.end()) {
-            p.mine = std::make_shared<Blob>();
-            p.mine->digest = p.d; p.mine->size = size;
-            p.mine->on_disk = p.mine->spill_done = true;
-            p.mine->sidecar.swap(side);
-            e->blobs[p.d] = p.mine;
+            L.mine = std::make_shared<Blob>();
+            L.mine->digest = L.d; L.mine->size = size;
+            L.mine->on_disk = L.mine->spill_done = true;
+            L.mine->sidecar = side;
+            e->blobs[L.d] = L.mine;
         }
     }
-    if (in_hbm) { close(fd); stream_abort_impl(e, id); return DM_OK; }
-    p.tiny = size <= e->tiny_max;
-    for (uint64_t off = 0; p.tiny && rc == DM_OK && off < size;) {
+    if (in_hbm) { shut(); stream_abort_impl(e, id); return DM_OK; }
+    std::shared_ptr<Stream> sp = find_stream(e, id);
+    { std::lock_guard<std::mutex> g(sp->mu); sp->load = true; }
+    L.stream = id;
+    L.tiny = size <= e->tiny_max;
+    {
+        std::lock_guard<std::mutex> g(L.mu);
+        L.sp = sp;
+        L.size = size;
+        L.side.swap(side);
+        L.opened = true;
+    }
+    L.cv.notify_all();
+    return 1;
+}
+
+// Read the file of an opened load into its stream and close it: a tiny one into the stream's private buffer (flushed
+// here when `flush_tiny`, else by the caller), anything else through acquired ring windows, flushed.  DM_OK, or the
+// load's final status (its stream aborted, the entry it registered taken back).
+int load_fill(dm_engine *e, Load &L, uint8_t *tiny_buf, bool flush_tiny)
+{
+    const uint64_t size = L.size;
+    const uint64_t id = L.stream;
+    int rc = DM_OK;
+    for (uint64_t off = 0; L.tiny && rc == DM_OK && off < size;) {
         ssize_t got;
-        do got = pread(fd, tiny_buf + off, size - off, (off_t)off); while (got < 0 && errno == EINTR);
+        do got = pread(L.fd, tiny_buf + off, size - off, (off_t)off); while (got < 0 && errno == EINTR);
         if (got <= 0) { rc = fail(DM_EIO, "could not read the disk tier file"); break; }
         off += (uint64_t)got;
         if (off == size) rc = stream_write_impl(e, id, tiny_buf, size);
     }
-    for (uint64_t off = 0; !p.tiny && rc == DM_OK && off < size;) {
+    for (uint64_t off = 0; !L.tiny && rc == DM_OK && off < size;) {
+        if (e->load_stop) { rc = fail(DM_ESTATE, "the engine is being destroyed"); break; }
         void *win = nullptr;
         size_t cap = 0;
         rc = stream_acquire_impl(e, id, &win, &cap);
         if (rc != DM_OK) break;
         const size_t want = (size_t)std::min<uint64_t>(cap, size - off);
         ssize_t got;
-        do got = pread(fd, win, want, (off_t)off); while (got < 0 && errno == EINTR);
+        do got = pread(L.fd, win, want, (off_t)off); while (got < 0 && errno == EINTR);
         if (got <= 0) {                                  // a read error, or the file shrank while it was read
             stream_commit_impl(e, id, 0);
             rc = fail(DM_EIO, "could not read the disk tier file");
@@ -1348,29 +1394,171 @@ int promote_start(dm_engine *e, Promotion &p, uint8_t *tiny_buf, bool may_open)
         rc = stream_commit_impl(e, id, (size_t)got);
         off += (uint64_t)got;
     }
-    close(fd);
-    if (rc == DM_OK && !p.tiny) rc = stream_flush_impl(e, id);
-    if (rc != DM_OK) { stream_abort_impl(e, id); promote_undo(e, p); return rc; }
-    p.stream = id;
-    return 1;
+    close(L.fd);
+    L.fd = -1;
+    if (rc == DM_OK && (!L.tiny || flush_tiny)) rc = stream_flush_impl(e, id);
+    if (rc != DM_OK) { stream_abort_impl(e, id); load_undo(e, L); }
+    return rc;
 }
 
-int promote_verdict(dm_engine *e, Promotion &p)
+// Collect the verdict of a load whose stream is flushed (waits for it): DM_OK with the blob in HBM, DM_ECORRUPT with
+// the file dropped, or the error of a failed copy or launch (the file left untouched).
+int load_verdict(dm_engine *e, Load &L)
 {
     uint8_t got[32];
     int matched = 0;
-    const int rc = stream_finish_impl(e, p.stream, got, &matched);
+    const int rc = stream_finish_impl(e, L.stream, got, &matched);
     if (rc != DM_OK) {
-        stream_abort_impl(e, p.stream);                  // (an id finish released just says so)
-        promote_undo(e, p);
+        stream_abort_impl(e, L.stream);                  // (an id finish released just says so)
+        load_undo(e, L);
         return rc;
     }
     if (matched) return DM_OK;
-    drop_corrupt(e, p.d, p.seen);
+    drop_corrupt(e, L.d, L.seen);
     return DM_ECORRUPT;
 }
 
+// The end of a load dm_cache_open_verified began: its slot reservation and disk-tier pin go, a verified blob counts as
+// used, and the load ends.
+void load_release(dm_engine *e, Load &L, int status)
+{
+    const std::string why = status == DM_ECORRUPT ? kCorruptText : g_last_error;
+    if (L.reserved) { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved--; L.reserved = false; }
+    if (status == DM_OK) tier_touch(e, L.d);
+    tier_unpin(e, L.d);
+    load_end(e, L, status, why.c_str());
+}
+
+// A loader thread: reads opened loads' files into their streams, and collects the verdicts of loads whose streams
+// have completed.  Verdicts go first: they are quick, and readers wait for them.  One thread scans load_wait at a time:
+// a load it has taken out of the list is invisible to the others, so a kick that arrives meanwhile stays set for the
+// scanner's next round rather than being spent on a scan that cannot see that load.
+void load_main(dm_engine *e)
+{
+    cudaSetDevice(e->device);
+    std::vector<uint8_t> tiny_buf(e->tiny_max);
+    std::unique_lock<std::mutex> g(e->load_mu);
+    for (;;) {
+        e->load_cv.wait(g, [&] { return e->load_stop || (e->load_kick && !e->load_scanning) || !e->load_q.empty(); });
+        if (e->load_stop) return;
+        if (e->load_kick && !e->load_scanning) {
+            e->load_kick = false;
+            e->load_scanning = true;
+            std::vector<std::shared_ptr<Load>> wait, rest;
+            wait.swap(e->load_wait);
+            g.unlock();
+            for (auto &L : wait) {
+                bool over;
+                { std::lock_guard<std::mutex> gs(L->sp->mu); over = L->sp->st == St::Done || L->sp->st == St::Aborted; }
+                if (over) load_release(e, *L, load_verdict(e, *L));
+                else rest.push_back(std::move(L));
+            }
+            g.lock();
+            e->load_wait.insert(e->load_wait.end(), rest.begin(), rest.end());
+            e->load_scanning = false;
+            continue;
+        }
+        std::shared_ptr<Load> L = std::move(e->load_q.front());
+        e->load_q.pop_front();
+        g.unlock();
+        const int rc = load_fill(e, *L, tiny_buf.data(), true);
+        if (rc != DM_OK) load_release(e, *L, rc);
+        g.lock();
+        if (rc == DM_OK) {
+            e->load_wait.push_back(std::move(L));
+            e->load_kick = true;                         // its stream may have completed already
+        }
+    }
+}
+
+// Claim and start the load of a promotion: DM_OK when the blob is in HBM, 1 when its stream is open and filled (flushed
+// unless tiny), 2 when another load of the digest runs (its verdict is collected at the end of the call), or the
+// promotion's final status.
+int promote_start(dm_engine *e, Promotion &p, uint8_t *tiny_buf, bool may_open)
+{
+    int rc;
+    { std::lock_guard<std::mutex> g(e->mu); rc = load_claim(e, p.d, &p.load); }
+    if (rc != 1) return rc;
+    p.own = true;
+    Load &L = *p.load;
+    rc = load_open(e, L, may_open);
+    if (rc == 1 && (rc = load_fill(e, L, tiny_buf, false)) == DM_OK) return 1;
+    load_end(e, L, rc, g_last_error.c_str());
+    return rc;
+}
+
 }  // namespace
+
+}  // extern "C"
+
+namespace dmi {
+
+int load_claim(dm_engine *e, const Digest &d, std::shared_ptr<Load> *L)
+{
+    auto it = e->blobs.find(d);
+    if (it != e->blobs.end() && it->second->in_hbm) return DM_OK;
+    std::shared_ptr<Load> &slot = e->loads[d];
+    if (slot) { *L = slot; return 2; }
+    slot = std::make_shared<Load>();
+    slot->d = d;
+    *L = slot;
+    return 1;
+}
+
+int load_begin(dm_engine *e, const std::shared_ptr<Load> &L)
+{
+    // one slot of the reservation promotions, checks and imports share: at most half of the free slots nobody has
+    // spoken for, so none with one or none left, which stays dm_stream_open's
+    {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        const size_t free = e->free_slots.size();
+        L->reserved = free > e->promote_reserved && (free - e->promote_reserved) / 2 >= 1;
+        if (L->reserved) e->promote_reserved++;
+    }
+    tier_pin(e, L->d);                                   // not a disk-tier victim until its verdict
+    const int rc = load_open(e, *L, L->reserved);
+    if (rc != 1) { load_release(e, *L, rc); return rc; }
+    {
+        std::lock_guard<std::mutex> g(e->load_mu);
+        if (e->loaders.empty())
+            for (int i = 0; i < kLoadThreads; ++i) e->loaders.emplace_back(load_main, e);
+        e->load_q.push_back(L);
+    }
+    e->load_cv.notify_all();
+    return 1;
+}
+
+void load_wake(dm_engine *e)
+{
+    { std::lock_guard<std::mutex> g(e->load_mu); e->load_kick = true; }
+    e->load_cv.notify_all();
+}
+
+void load_stop_all(dm_engine *e)
+{
+    std::vector<std::thread> th;
+    {
+        std::lock_guard<std::mutex> g(e->load_mu);
+        e->load_stop = true;
+        th.swap(e->loaders);
+    }
+    e->load_cv.notify_all();
+    for (auto &t : th) t.join();
+    // loads nobody will read in or collect: their files close, and whoever waits for them wakes (their streams go with
+    // the engine)
+    std::vector<std::shared_ptr<Load>> left(e->load_q.begin(), e->load_q.end());
+    left.insert(left.end(), e->load_wait.begin(), e->load_wait.end());
+    e->load_q.clear();
+    e->load_wait.clear();
+    for (auto &L : left) {
+        if (L->fd >= 0) { close(L->fd); L->fd = -1; }
+        load_end(e, *L, DM_ESTATE, "the engine was destroyed before the load's verdict");
+    }
+}
+
+}  // namespace dmi
+
+extern "C" {
 
 static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
 {
@@ -1406,22 +1594,27 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
         std::deque<Promotion *> open;                    // verdict not collected yet (oldest first)
         std::vector<Promotion *> unflushed;              // tiny ones among them, flushed together
         // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
-        auto flush = [&] { for (Promotion *p : unflushed) stream_flush_impl(e, p->stream); unflushed.clear(); };
+        auto flush = [&] { for (Promotion *p : unflushed) stream_flush_impl(e, p->load->stream); unflushed.clear(); };
+        auto settle = [&](Promotion &p) {
+            p.status = load_verdict(e, *p.load);
+            load_end(e, *p.load, p.status, p.status == DM_ECORRUPT ? kCorruptText : g_last_error.c_str());
+        };
         for (size_t k; (k = next.fetch_add(1)) < work.size();) {
             if (open.size() >= per_thread) {
                 flush();
-                open.front()->status = promote_verdict(e, *open.front());
+                settle(*open.front());
                 open.pop_front();
             }
             Promotion &p = work[k];
             const int rc = promote_start(e, p, tiny_buf.data(), budget > 0);
+            if (rc == 2) continue;                       // another load's: collected below
             if (rc != 1) { p.status = rc; continue; }
             open.push_back(&p);
-            if (p.tiny) unflushed.push_back(&p);
+            if (p.load->tiny) unflushed.push_back(&p);
             if (unflushed.size() >= kPromoteTinyBatch) flush();
         }
         flush();
-        for (Promotion *p : open) p->status = promote_verdict(e, *p);
+        for (Promotion *p : open) settle(*p);
     };
     for (Promotion &p : work) tier_pin(e, p.d);        // held by this call: not disk-tier victims until it returns
     std::vector<std::thread> th;
@@ -1429,6 +1622,8 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
     if (nthreads) loader();
     for (auto &t : th) t.join();
     { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved -= budget; }
+    for (Promotion &p : work)                          // a load that was already running reports its own verdict
+        if (p.load && !p.own) p.status = load_wait(*p.load);
     for (Promotion &p : work) {
         if (p.status == DM_OK) tier_touch(e, p.d);
         tier_unpin(e, p.d);

@@ -1,4 +1,4 @@
-// C-ABI, part 2: hit serving (readers, followers), device-resident ingest, the synthetic generator.
+// C-ABI, part 2: hit serving (readers, followers, verified opens), device-resident ingest, the synthetic generator.
 #include "engine_internal.hpp"
 
 extern "C" {
@@ -59,6 +59,62 @@ static int cache_open_impl(dm_engine *e, const uint8_t digest[32], uint64_t *rea
             fclose(mf);
         }
     }
+    const uint64_t id = e->next_id.fetch_add(1);
+    {
+        std::lock_guard<std::mutex> g(e->reader_mu[id % kStripes]);
+        e->readers[id % kStripes][id] = r;
+    }
+    *reader = id;
+    if (size) *size = r->size;
+    return DM_OK;
+}
+
+// A blob in HBM opens as with dm_cache_open.  One on the disk tier only is loaded into a fresh HBM extent and hashed
+// there (struct Load), and the reader follows the load's stream; a load of the digest that is already running is
+// followed instead of starting another.
+static int cache_open_verified_impl(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size)
+{
+    if (!e || !digest || !reader) return fail(DM_EINVAL, "null argument");
+    if (e->cfg.flags & DM_F_NO_HBM_CAS) return fail(DM_ESTATE, "the engine has no HBM tier (DM_F_NO_HBM_CAS)");
+    Digest d;
+    memcpy(d.b, digest, 32);
+    auto r = std::make_shared<Reader>();
+    // more than one round only when a load ends in HBM between two looks (a stream published the blob meanwhile)
+    for (int round = 0; round < 8 && !r->blob && !r->load; ++round) {
+        std::shared_ptr<Load> L;
+        int claim;
+        {
+            std::lock_guard<std::mutex> g(e->mu);
+            if (e->cas_dir.empty()) {
+                auto it = e->blobs.find(d);
+                if (it == e->blobs.end() || !it->second->in_hbm) return DM_ENOENT;
+            }
+            claim = load_claim(e, d, &L);
+            if (claim == DM_OK) {                        // verified when it entered HBM: an ordinary hit
+                r->blob = e->blobs.find(d)->second;
+                r->blob->readers++;
+                lru_touch(e, r->blob.get());
+                r->size = r->blob->size;
+                break;
+            }
+        }
+        if (claim == 1) {
+            const int rc = load_begin(e, L);
+            if (rc == DM_OK) continue;
+            if (rc != 1) return rc;
+        }
+        std::unique_lock<std::mutex> g(L->mu);
+        L->cv.wait(g, [&] { return L->opened || L->done; });
+        if (!L->opened) {                                // that load ended before its stream opened
+            if (L->status == DM_OK) continue;
+            return L->status == DM_ENOENT ? DM_ENOENT : fail(L->status, L->why.c_str());
+        }
+        r->load = L;
+        r->follow = L->sp;
+        r->size = L->size;
+        r->disk_meta = L->side;
+    }
+    if (!r->blob && !r->load) return fail(DM_ENOENT, "the blob kept leaving HBM while it was opened");
     const uint64_t id = e->next_id.fetch_add(1);
     {
         std::lock_guard<std::mutex> g(e->reader_mu[id % kStripes]);
@@ -138,24 +194,60 @@ static int follow_disk_read(dm_engine *e, Reader *r, uint64_t off, void *buf, si
     return DM_OK;
 }
 
+// The verdict of the load a verified reader follows (dm_cache_open_verified): on a match the reader becomes an
+// ordinary HBM reader of the blob the load published (returns 1), otherwise every read returns the load's failure.
+// Reader mutex held.
+static int load_switch(dm_engine *e, Reader *r)
+{
+    Load *L = r->load.get();
+    int status;
+    std::string why;
+    {
+        std::unique_lock<std::mutex> g(L->mu);
+        L->cv.wait(g, [&] { return L->done; });
+        status = L->status;
+        why = L->why;
+    }
+    if (status != DM_OK) return fail(status, why.c_str());
+    std::lock_guard<std::mutex> g(e->mu);
+    auto it = e->blobs.find(L->d);
+    if (it == e->blobs.end() || !it->second->in_hbm)
+        return fail(DM_ESTATE, "the verified blob was evicted from HBM before this reader switched over to it: open it again");
+    r->blob = it->second;
+    r->blob->readers++;
+    r->size = r->blob->size;
+    r->disk_meta.clear();
+    r->follow.reset();
+    return 1;
+}
+
 // Read from a body that is still arriving (request coalescing).  Blocks until bytes past `off` have
 // been DMA'd, the body completes, or it fails.  Returns DM_OK with *nread set, a dm_err, or 1 when the
 // body has completed and been published (the reader has been switched to the blob; caller continues).
+// A verified reader (r->load) follows its load's stream the same way, except that its last byte, and its EOF, wait
+// for the load's verdict: no read hands out a whole body that has not been verified.
 static int follow_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t len, size_t *nread)
 {
     std::lock_guard<std::mutex> gr(r->mu);
     if (!r->follow) return 1;
     Stream *s = r->follow.get();
     if (s->disk) return follow_disk_read(e, r, off, buf, len, nread);
+    const bool verified = r->load != nullptr;
+    const uint64_t gate = verified ? (r->size ? r->size - 1 : 0) : UINT64_MAX;     // bytes from here on wait for the verdict
     std::vector<std::pair<uint8_t *, uint64_t>> segs;
     size_t n = 0;
     {
         std::unique_lock<std::mutex> g(s->mu);
         s->followers++;
         s->cv.wait(g, [&] {
-            return s->st == St::Done || s->st == St::Aborted || (off < s->dma_issued && !s->completing) || len == 0;
+            return s->st == St::Done || s->st == St::Aborted || (off < std::min(s->dma_issued, gate) && !s->completing) ||
+                   (len == 0 && (!verified || off < r->size));
         });
         s->followers--;
+        if (verified && (s->st == St::Done || s->st == St::Aborted)) {
+            g.unlock();
+            return load_switch(e, r);
+        }
         if (s->st == St::Aborted) return fail(DM_ESTATE, "the upstream body this reader followed was aborted");
         if (s->st == St::Done) {
             std::shared_ptr<Blob> b = s->blob;
@@ -170,7 +262,7 @@ static int follow_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t 
             return 1;
         }
         if (len == 0) return DM_OK;
-        n = (size_t)std::min<uint64_t>(len, s->dma_issued - off);
+        n = (size_t)std::min<uint64_t>(len, std::min(s->dma_issued, gate) - off);
         for_segments(e, s->extents, off, n, [&](uint8_t *dev, uint64_t l) { segs.emplace_back(dev, l); });
         s->follow_reads++;                      // pins the extents until the copy-out below is done
     }
@@ -438,6 +530,7 @@ static int cache_device_extents_impl(dm_engine *e, uint64_t reader, void **dev_p
     if (!e) return fail(DM_EINVAL, "null argument");
     std::shared_ptr<Reader> r = find_reader(e, reader);
     if (!r) return fail(DM_EINVAL, "unknown reader id");
+    if (!r->blob && r->load) return fail(DM_ESTATE, "the blob is still being loaded and verified: read it to its end first");
     if (!r->blob) return fail(DM_ESTATE, "blob is on the disk tier only");
     const auto &ext = r->blob->extents;
     uint64_t left = r->blob->size;
@@ -873,6 +966,7 @@ int dm_synth_fill_device_many(dm_engine *e, uint64_t seed, uint64_t first_blob, 
 
 // ---- exported wrappers: file the error text under the reader id (dm_error_detail) ----
 int dm_cache_open(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_impl(e, digest, reader, size)); }
+int dm_cache_open_verified(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_verified_impl(e, digest, reader, size)); }
 int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t len, size_t *nread) { return note_err(e, reader, cache_read_impl(e, reader, off, buf, len, nread)); }
 int dm_cache_meta(dm_engine *e, uint64_t reader, char *buf, size_t cap, size_t *len) { return note_err(e, reader, cache_meta_impl(e, reader, buf, cap, len)); }
 int dm_cache_close(dm_engine *e, uint64_t reader) { return note_err(e, reader, cache_close_impl(e, reader)); }

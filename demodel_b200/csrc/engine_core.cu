@@ -693,8 +693,10 @@ void complete_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, const uint
     g.lock();
     s->blob = b;
     s->st = St::Done;
+    const bool load = s->load;
     g.unlock();
     s->cv.notify_all();
+    if (load) load_wake(e);
 }
 
 void completer_main(dm_engine *e)

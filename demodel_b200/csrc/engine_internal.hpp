@@ -1,9 +1,10 @@
 // engine_internal.hpp - types, constants and internal entry points shared by the engine's translation units:
 //   engine_core.cu    extents, ring slabs, CAS commit / eviction, the pump (launch decisions), the disk tier
 //   engine_api.cu     C-ABI: engine lifecycle, streams (ingest, ranges, checkpoint / resume, zero-copy windows),
-//                     promotion of disk-tier blobs back into HBM, checks of disk-tier files and imports of files from
-//                     outside the cache (internal streams), the listing of the disk tier
-//   engine_cache.cu   C-ABI: hit serving (readers, followers), device-resident ingest, the synthetic generator
+//                     loads of disk-tier blobs back into HBM (promotion, verified opens), checks of disk-tier files and
+//                     imports of files from outside the cache (internal streams), the listing of the disk tier
+//   engine_cache.cu   C-ABI: hit serving (readers, followers, verified opens), device-resident ingest, the synthetic
+//                     generator
 // Not installed, not part of the boundary (that is include/demodel_b200.h).
 #pragma once
 #include "../../include/demodel_b200.h"
@@ -207,6 +208,7 @@ struct Stream {
     std::shared_ptr<Pack> pack;      // tiny body travelling in a shared pack: [pack_off, pack_off + pack_len) of pack->dev
     uint32_t pack_off = 0, pack_len = 0;
     std::vector<std::pair<std::string, std::string>> meta;   // dm_stream_set_meta
+    bool load = false;         // the stream of a Load run by the loader threads: its completion wakes them (load_wake)
     uint32_t followers = 0;    // readers attached while the body is still arriving (request coalescing)
     uint32_t follow_reads = 0; // followers' copy-outs in flight: the extents must not be freed or handed over meanwhile
     bool completing = false;   // digest known, extents being handed to the index: followers wait for Done
@@ -224,13 +226,37 @@ struct Stream {
     std::shared_ptr<Blob> blob;   // set at commit
 };
 
+// A disk-tier blob being loaded into a fresh HBM extent and hashed there as an internal stream whose expected digest is
+// its name (dm_cache_promote, dm_cache_open_verified).  e->loads indexes the running ones by digest, so that a digest is
+// never loaded twice at once: a verified open attaches its reader to the running load, a promotion waits for its verdict.
+struct Load {
+    Digest d;
+    // the thread that runs the load: set before `opened`, not touched by anybody else
+    int fd = -1;                          // the tier file, open from load_open until load_fill has read it
+    struct stat seen{};                   // the file that was read (st_dev / st_ino)
+    std::shared_ptr<Blob> mine;           // the disk-only entry this load registered (none if one existed)
+    uint64_t stream = 0;
+    bool tiny = false;                    // at most tiny_max bytes: read into the stream's private buffer
+    bool reserved = false;                // holds one slot of promote_reserved (a verified open's load)
+    // published under mu: readers wait here for the stream to open and for the verdict
+    std::mutex mu;
+    std::condition_variable cv;
+    std::shared_ptr<Stream> sp;           // the load's stream (readers follow it)
+    uint64_t size = 0;
+    std::string side;                     // the sidecar text read at open
+    bool opened = false, done = false;
+    int status = DM_OK;                   // once done: DM_OK (the blob is in HBM) or why the load failed
+    std::string why;
+};
+
 struct Bounce;
 struct Window { Bounce *b = nullptr; uint64_t off = 0, len = 0; bool pending = false; };
 
 struct Reader {
     std::shared_ptr<Blob> blob;
-    std::string disk_meta;        // sidecar text, disk-tier readers
+    std::string disk_meta;        // sidecar text, disk-tier readers (and verified readers until the verdict)
     std::shared_ptr<Stream> follow;   // in-flight body this reader is coalesced onto (until it completes)
+    std::shared_ptr<Load> load;       // dm_cache_open_verified of a disk-tier blob: the load `follow` belongs to
     int fd = -1;                  // disk tier; a follower of a disk-backed body: its own descriptor of the body's file
     Digest disk_digest{};         // ... the blob it reads
     bool disk_pin = false;        // ... pinned against disk-tier eviction until dm_cache_close
@@ -402,6 +428,18 @@ struct dm_engine {
     bool disk_stop = false;
     std::vector<std::thread> disk_threads;
 
+    // Loads of disk-tier blobs (struct Load).  `loads` is guarded by mu.  The loader threads (started by the first
+    // dm_cache_open_verified that needs one) read opened loads' files into their streams (load_q) and collect the verdicts
+    // of those being hashed (load_wait) when a load stream completes (load_kick).
+    std::unordered_map<Digest, std::shared_ptr<Load>, DigestHash> loads;
+    std::mutex load_mu;
+    std::condition_variable load_cv;
+    std::deque<std::shared_ptr<Load>> load_q;
+    std::vector<std::shared_ptr<Load>> load_wait;
+    bool load_kick = false, load_scanning = false;
+    std::atomic<bool> load_stop{false};
+    std::vector<std::thread> loaders;
+
     std::mutex bounce_mu;
     std::condition_variable bounce_cv;
     std::vector<Bounce *> bounce_free;
@@ -540,6 +578,16 @@ void alias_load(dm_engine *e);                // dm_engine_create: replay <cas_d
 bool digest_from_hex(const char *hex, uint8_t out[32]);
 bool alias_key_ok(const char *key);           // 1..4096 bytes without control characters: one line of aliases.log
 void sweep_incoming(const std::string &dir);  // remove files under incoming/ of processes that are gone
+
+// Loads of disk-tier blobs (engine_api.cu).
+// e->mu held: DM_OK when `d` is in HBM, 1 when *L is a new load the caller runs (every outcome must reach load_end),
+// 2 when *L is a load of `d` that is already running.
+int load_claim(dm_engine *e, const Digest &d, std::shared_ptr<Load> *L);
+// dm_cache_open_verified: run a claimed load.  Its stream is opened on the calling thread, the file is read in and the
+// verdict collected by the loader threads.  1: running; otherwise the load's final status (it has ended).
+int load_begin(dm_engine *e, const std::shared_ptr<Load> &L);
+void load_wake(dm_engine *e);                 // a load's stream completed (complete_stream)
+void load_stop_all(dm_engine *e);             // dm_engine_destroy, while the pump still runs
 
 // Disk-tier limit (engine_core.cu).  None takes a stream mutex or may be called with e->mu held.  With no limit set
 // they only count pins; reservations always succeed and nothing is stat'ed, touched or written.

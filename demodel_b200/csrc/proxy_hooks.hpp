@@ -267,9 +267,11 @@ private:
 
 class HitReader {
 public:
-    HitReader(dm_engine *e, const uint8_t digest[32]) : e_(e)
+    // verified: Pool.HitVerified (dm_cache_open_verified): a disk-tier blob is served only as the GPU verifies it, and
+    // Read returns DM_ECORRUPT / DM_EIO / DM_ECUDA instead of its last byte when it does not hash to its name.
+    HitReader(dm_engine *e, const uint8_t digest[32], bool verified = false) : e_(e)
     {
-        rc_ = dm_cache_open(e, digest, &id_, &size_);
+        rc_ = verified ? dm_cache_open_verified(e, digest, &id_, &size_) : dm_cache_open(e, digest, &id_, &size_);
         open_ = rc_ == DM_OK;
     }
     // By request URL: a digest in the URL (OCI) or the alias index (HuggingFace resolve/ URLs).

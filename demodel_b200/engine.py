@@ -199,6 +199,22 @@ class Engine:
         check(rc, "dm_cache_open")
         return rid.value, size.value
 
+    def cache_open_verified(self, digest: bytes) -> Optional[tuple[int, int]]:
+        """dm_cache_open that never serves an unverified disk-tier blob: (reader, size) or None on a miss.
+
+        A blob in HBM opens as with cache_open.  One on the disk tier only is loaded into HBM and hashed there while
+        the reader is served from the loaded bytes; the read of the last byte (and the EOF read) waits for the verdict.
+        A mismatch makes that read and every later one raise DM_ECORRUPT (file and sidecar are removed); DM_EIO and
+        DM_ECUDA likewise.  Raises DM_ENOMEM when the blob cannot be loaded (larger than the arena, no room, no
+        slot: cache_open still serves it), DM_ECORRUPT when the file is not its sidecar's size, DM_ESTATE on an
+        engine without an HBM tier."""
+        rid, size = C.c_uint64(), C.c_uint64()
+        rc = self._lib.dm_cache_open_verified(self._h, _digest_arg(digest), C.byref(rid), C.byref(size))
+        if rc == DM_ENOENT:
+            return None
+        check(rc, "dm_cache_open_verified")
+        return rid.value, size.value
+
     def cache_follow(self, digest: bytes) -> Optional[tuple[int, int]]:
         """Attach to a body that is still being ingested (request coalescing): (reader, size_hint) or None.
 

@@ -307,6 +307,28 @@ func (p *Pool) Hit(digest *[32]byte) *HitReader {
 	return &HitReader{e: e, id: id, Size: int64(size)}
 }
 
+// HitVerified is Hit that never serves a disk-tier blob the GPU has not
+// verified (dm_cache_open_verified).  A blob in HBM opens as with Hit; one on
+// the disk tier only is loaded into HBM and hashed there while it is served
+// from the loaded bytes.  Size is the blob's size (send it as Content-Length):
+// the Read that would return the last byte waits for the verdict, and on a
+// mismatch (DM_ECORRUPT), a failed read of the file (DM_EIO) or a failed copy
+// or launch (DM_ECUDA) Read returns an *Error instead, so net/http cuts the
+// response short and the client never receives a whole body that does not
+// hash to its name.  nil on a miss, and when the blob cannot be loaded
+// (DM_ENOMEM: larger than the arena, no room, no stream slot to spare;
+// DM_ESTATE: a pool without an HBM tier); Hit still serves those, unverified,
+// for a caller that accepts that.
+func (p *Pool) HitVerified(digest *[32]byte) *HitReader {
+	e := p.engineFor(digest)
+	var id, size C.uint64_t
+	rc := C.dm_cache_open_verified(e, (*C.uint8_t)(unsafe.Pointer(&digest[0])), &id, &size)
+	if rc != C.DM_OK {
+		return nil
+	}
+	return &HitReader{e: e, id: id, Size: int64(size)}
+}
+
 func (r *HitReader) Read(p []byte) (int, error) {
 	if len(p) == 0 {
 		return 0, nil

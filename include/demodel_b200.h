@@ -50,7 +50,8 @@ typedef enum dm_err {
     DM_EIO       = -6,   /* on-disk CAS tier I/O error */
     DM_ENODEV    = -7,   /* no CUDA device / device ordinal out of range */
     DM_ERANGE    = -8,   /* offset beyond blob end */
-    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote, dm_cache_verify), or a file
+    DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote, dm_cache_verify,
+                          * dm_cache_open_verified and its reads), or a file
                           * to import does not hash to its expected digest (dm_cache_import) */
 } dm_err;
 
@@ -225,6 +226,42 @@ int dm_stream_abort(dm_engine *e, uint64_t id);
 /* ---- hit serving: OnRequest short-circuit (start.go:197-200) ----------- */
 int dm_cache_contains(dm_engine *e, const uint8_t digest[32], uint64_t *size);  /* DM_ENOENT on miss */
 int dm_cache_open(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size);
+/* dm_cache_open that never serves a disk-tier blob it has not verified.  Returns at once, without waiting for a load.
+ *   in HBM       exactly dm_cache_open (those bytes were verified when they entered HBM), LRU touch included
+ *   disk only    the file is loaded into a fresh HBM extent and hashed there, as dm_cache_promote loads it, and the
+ *                reader is served from that extent as the bytes land: the same bytes the kernel hashes, never a second
+ *                read of the file.  *size is the file's size, checked against its sidecar.  The stream and its extent
+ *                (evicting HBM LRU blobs) are set up on the calling thread; the file is read in and the verdict is
+ *                collected by engine threads.  A load of the digest that is already running (another verified open, a
+ *                dm_cache_promote) is followed instead: a digest is never loaded twice at once.
+ * dm_cache_read on a reader whose load has no verdict yet blocks until bytes past `off` have landed in the extent, and
+ * NO read returns byte size - 1, nor the EOF at off == size, before the verdict: a caller that sent Content-Length from
+ * *size never completes a body that does not hash to its name (on an error it closes the connection, and the client
+ * sees a short body).  A blob of at most 64 KiB travels in a pack and lands in HBM together with its verdict: every
+ * read of it waits for the verdict.  Then:
+ *   verified     the reader is an ordinary HBM reader (it pins the blob; dm_cache_device_extents works, dm_cache_meta
+ *                returns the sidecar's text unchanged).  The blob stays in HBM, as if promoted, also when every reader
+ *                closed before the verdict.  Before it, dm_cache_meta returns the sidecar read at open and
+ *                dm_cache_device_extents DM_ESTATE
+ *   mismatch     that read and every later one return DM_ECORRUPT (dm_error_detail(reader) says why); file and sidecar
+ *                are removed if the path still names the file that was read, and the digest is a miss
+ *   DM_EIO       the file could not be read or shrank; DM_ECUDA: a copy or launch failed.  The file is left untouched
+ *                and the blob is not in HBM
+ * Every outcome wakes blocked readers; dm_cache_close never aborts a load.  The load pins the digest against disk-tier
+ * eviction until its verdict, and a verified load is a use of the blob.  bytes_hashed and h2d_bytes grow by the blob
+ * once however many readers follow it; bytes_served by what they read.  dm_cache_follow does not see loads.
+ * A load holds ring slabs only while it fills them: a reader that stops reading holds none, and no stream slot once the
+ * verdict is in.
+ * Errors (nothing is opened, the file is left untouched unless DM_ECORRUPT):
+ *   DM_ENOENT    on neither tier (a body still being ingested too: dm_cache_follow attaches to those)
+ *   DM_ECORRUPT  the file is not the size its sidecar states: file and sidecar removed
+ *   DM_EIO       the file could not be opened
+ *   DM_ENOMEM    larger than hbm_cas_bytes, no room even after LRU eviction, or no stream slot to spare (the budget
+ *                dm_cache_promote, dm_cache_verify and dm_cache_import share): dm_cache_open still serves it, unverified
+ *   DM_ESTATE    the engine has no HBM tier (DM_F_NO_HBM_CAS); DM_EINVAL: bad arguments
+ * Verified serving finishes at one SHA-256 chain's rate per blob (DESIGN.md section 7), where dm_cache_open reads the
+ * file at memory speed. */
+int dm_cache_open_verified(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size);
 int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t len, size_t *nread);
 /* The blob's sidecar as JSON text: {"digest":"sha256:..","size":N,"encoding":"identity",
  * ..,"headers":{..}}.  *len receives the full length; up to cap-1 bytes + NUL are copied. */
@@ -233,7 +270,7 @@ int dm_cache_close(dm_engine *e, uint64_t reader);
 int dm_cache_evict(dm_engine *e, const uint8_t digest[32]);   /* HBM tier only; disk copy stays */
 /* Bring cached blobs back into HBM, verifying each disk copy on the GPU as it loads.  A blob leaves HBM when it is
  * evicted or the engine restarts, and dm_cache_open serves it from <cas_dir>/blobs/ from then on, unverified and
- * without dm_cache_device_extents.  This reads each file into the pinned ring, DMAs it into a fresh HBM extent and
+ * without dm_cache_device_extents (dm_cache_open_verified loads it the same way on a hit).  This reads each file into the pinned ring, DMAs it into a fresh HBM extent and
  * hashes it there as an ordinary stream with the digest as its expected value; many files load at once, so their
  * hash chains share launches.  Blocks until every status is known.  status_out[i]:
  *   DM_OK        it was in HBM when the call looked, or its disk copy was loaded and hashed to digests[i].  HBM is
@@ -249,7 +286,9 @@ int dm_cache_evict(dm_engine *e, const uint8_t digest[32]);   /* HBM tier only; 
  * A file is removed only if its path still names the file that was read (one a stream published meanwhile stays).
  * A disk reader that opened a corrupt file before keeps its descriptor and reads what the file holds.  The file and
  * sidecar of a verified blob stay as they are (nothing is written back), and dm_cache_meta returns the sidecar's text
- * unchanged; a blob without a sidecar is promoted with no headers.  Duplicates in digests[] are loaded once.  The
+ * unchanged; a blob without a sidecar is promoted with no headers.  Duplicates in digests[] are loaded once, and a
+ * digest whose load is already running (dm_cache_open_verified, another promotion) is not loaded again: its status is
+ * that load's verdict, waited for.  The
  * call opens at most half of the stream slots that are free when it starts and not reserved by other running calls,
  * so it never takes the last one from dm_stream_open; with fewer than two such slots it loads nothing, and each blob
  * it would have loaded is DM_ENOMEM.
