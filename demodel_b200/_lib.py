@@ -24,6 +24,8 @@ DM_ING_REPLACE = 0x2
 DM_ING_FORCE_WIDE = 0x4
 DM_ING_FORCE_DEEP = 0x8
 DM_IMP_LINK = 0x1
+DM_RM_ALIASES = 0x1
+DM_RM_PARTIAL = 0x2
 
 
 class DmConfig(C.Structure):
@@ -128,6 +130,7 @@ SIGNATURES = {
     "dm_cache_meta": (C.c_int, [_P, C.c_uint64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "dm_cache_close": (C.c_int, [_P, C.c_uint64]),
     "dm_cache_evict": (C.c_int, [_P, _P]),
+    "dm_cache_remove": (C.c_int, [_P, _P, C.c_uint32, C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_promote": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_verify": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_list": (C.c_int, [_P, _P, _P, _U64P, C.c_uint32, C.POINTER(C.c_uint32)]),
@@ -138,6 +141,9 @@ SIGNATURES = {
     "dm_cache_follow": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_alias_put": (C.c_int, [_P, C.c_char_p, _P]),
     "dm_cache_alias_get": (C.c_int, [_P, C.c_char_p, _P]),
+    "dm_cache_alias_del": (C.c_int, [_P, C.c_char_p]),
+    "dm_cache_alias_list": (C.c_int, [_P, C.c_char_p, C.c_char_p, _P, C.c_size_t, _P, C.c_uint32,
+                                      C.POINTER(C.c_uint32), C.POINTER(C.c_int)]),
     "dm_stream_suspend": (C.c_int, [_P, C.c_uint64, _U64P]),
     "dm_stream_resume_saved": (C.c_int, [_P, _P, C.c_uint64, _U64P, _U64P]),
     "dm_gunzip": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -400,8 +400,10 @@ int dm_engine_stats(dm_engine *e, dm_stats *o)
 // reads from offset 0, and nothing before resume_base is ever written.
 // `saved`: bytes of this body already counted in the disk tier (a saved download being resumed): a disk-backed stream
 // makes room only for the rest of its size_hint.
+// `internal`: the stream of a load (e->loads already keeps dm_cache_remove off its digest); any other stream with an
+// expected digest holds it (e->holds) until it is dropped.
 static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t size_hint, uint64_t *id, bool followable,
-                            uint64_t saved = 0)
+                            uint64_t saved = 0, bool internal = false)
 {
     if (!e || !id) return fail(DM_EINVAL, "null argument");
     auto sp = std::make_shared<Stream>();
@@ -454,6 +456,10 @@ static int stream_open_impl(dm_engine *e, const uint8_t expect[32], uint64_t siz
     if (size_hint && size_hint <= e->tiny_max && !sp->verify_only) {       // announced tiny: no ring slab (see Stream::small)
         sp->small.reset(new uint8_t[size_hint]);
         sp->small_cap = (uint32_t)size_hint;
+    }
+    if (sp->has_expect && !internal) {
+        sp->held = true;
+        hold_digest(e, sp->expect, "a stream opened with it as its expected digest");
     }
     {
         const int k = (int)(sp->id % kStripes);
@@ -901,6 +907,7 @@ static int stream_resume_saved_impl(dm_engine *e, const uint8_t expect[32], uint
     if (e->cas_dir.empty()) return DM_ENOENT;
     Digest d;
     memcpy(d.b, expect, 32);
+    DigestHold held(e, d, "dm_stream_resume_saved is taking its saved download over");
     tier_pin(e, d, true);                                // the saved download being taken over is not a victim
     const int rc = resume_saved_pinned(e, expect, size_hint, id, resume_from);
     tier_unpin(e, d, true);
@@ -1329,7 +1336,7 @@ int load_open(dm_engine *e, Load &L, bool may_open)
     if (size > e->cfg.hbm_cas_bytes) { shut(); return fail(DM_ENOMEM, "blob is larger than the HBM arena"); }
     if (!may_open) { shut(); return fail(DM_ENOMEM, "no stream slot to spare for a load of a disk tier blob"); }
     uint64_t id = 0;
-    int rc = stream_open_impl(e, L.d.b, size, &id, false);
+    int rc = stream_open_impl(e, L.d.b, size, &id, false, 0, true);
     if (rc != DM_OK) { shut(); return rc; }
     bool in_hbm = false;                                 // a stream published it meanwhile
     {
@@ -1616,6 +1623,7 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
         flush();
         for (Promotion *p : open) settle(*p);
     };
+    for (Promotion &p : work) hold_digest(e, p.d, "a running dm_cache_promote");
     for (Promotion &p : work) tier_pin(e, p.d);        // held by this call: not disk-tier victims until it returns
     std::vector<std::thread> th;
     for (size_t t = 1; t < nthreads; ++t) th.emplace_back(loader);
@@ -1627,6 +1635,7 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
     for (Promotion &p : work) {
         if (p.status == DM_OK) tier_touch(e, p.d);
         tier_unpin(e, p.d);
+        release_digest(e, p.d);
     }
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
     return DM_OK;
@@ -1847,6 +1856,7 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
         }
     }
     CheckRun run(e, work.size());
+    for (Check &c : work) hold_digest(e, c.d, "a running dm_cache_verify");
     for (Check &c : work) tier_pin(e, c.d);
     run.run(work,
             [&](Check &c, int *fd, std::string *path) -> int {
@@ -1859,6 +1869,7 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
             },
             [&](Check &c, int rc) -> int { return rc == 1 ? check_verdict(e, c) : rc; });
     for (Check &c : work) tier_unpin(e, c.d);
+    for (Check &c : work) release_digest(e, c.d);
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
     return DM_OK;
 }
@@ -2002,6 +2013,7 @@ int import_publish(dm_engine *e, Check &c, Import &im)
         dm_engine *e; Digest d;
         ~TierHold() { tier_unpin(e, d); }
     } hold{e, d};
+    DigestHold placing(e, d, "a running dm_cache_import is placing it");
     tier_pin(e, d);
     struct stat st;
     const bool placed = stat(dst.c_str(), &st) != 0;    // already in the disk tier: keep that copy, the staged one goes

@@ -451,8 +451,12 @@ static int cache_close_impl(dm_engine *e, uint64_t reader)
         }
     }
     if (r->blob) {
-        std::lock_guard<std::mutex> g(e->mu);
-        r->blob->readers--;
+        std::vector<Extent> gone;
+        {
+            std::lock_guard<std::mutex> g(e->mu);
+            gone = reader_gone(r->blob.get());
+        }
+        if (!gone.empty()) free_extents(e, gone);
     }
     if (r->fd >= 0) {
         close(r->fd);
@@ -542,11 +546,104 @@ static int cache_device_extents_impl(dm_engine *e, uint64_t reader, void **dev_p
     return (int)ext.size();
 }
 
+// ---- removal ------------------------------------------------------------------------
+
+}  // extern "C"
+
+namespace {
+
+// Remove one digest from both tiers.  tier_mu is held throughout, taken before e->mu as engine_internal.hpp orders, so
+// the DM_ESTATE checks and the removal are one decision: a load, promotion or disk-tier open that starts after it pins
+// the digest first (tier_mu) and then finds the files gone.
+int remove_one(dm_engine *e, const Digest &d, bool partial, std::string *why)
+{
+    std::lock_guard<std::mutex> gt(e->tier_mu);
+    bool found = false;
+    std::vector<Extent> ext;
+    {
+        std::unique_lock<std::mutex> g(e->mu);
+        const char *held = nullptr;
+        auto h = e->holds.find(d);
+        auto it = e->blobs.find(d);
+        if (h != e->holds.end()) held = h->second.what;
+        else if (e->loads.count(d)) held = "a running load into HBM (dm_cache_open_verified or dm_cache_promote)";
+        else if (it != e->blobs.end() && it->second->parked) held = "a running dm_ingest_device with DM_ING_REPLACE";
+        if (held) { *why = held; return DM_ESTATE; }
+        if (it != e->blobs.end()) {
+            std::shared_ptr<Blob> b = it->second;
+            found = b->in_hbm || b->on_disk;
+            e->blobs.erase(it);
+            lru_drop(e, b.get());
+            b->removed = true;                          // a queued spill skips it, a running one does not rename
+            b->in_hbm = false;
+            if (b->readers == 0) ext.swap(b->extents);  // otherwise the last dm_cache_close frees them
+            e->remove_cv.wait(g, [&] { return !b->renaming; });   // a spill moving its file into place: it goes below
+        }
+    }
+    if (!ext.empty()) free_extents(e, ext);
+    if (e->cas_dir.empty()) return found ? DM_OK : DM_ENOENT;
+    int rc = DM_OK;
+    auto gone = [&](const std::string &p) {
+        if (unlink(p.c_str()) == 0) return true;
+        if (errno != ENOENT && rc == DM_OK) { rc = DM_EIO; *why = "could not unlink " + p + ": " + strerror(errno); }
+        return false;
+    };
+    const std::string path = blob_path(e, d.b);
+    if (gone(path)) found = true;                       // the file, then its sidecar, as eviction removes them
+    if (rc == DM_OK) gone(path + ".meta");
+    if (partial && rc == DM_OK) {                       // the record, then its bytes
+        const std::string base = e->cas_dir + "/partial/" + hex_of(d.b, 32);
+        if (gone(base + ".ckpt")) { found = true; if (e->n_suspended) e->n_suspended--; }
+        if (rc == DM_OK && gone(base + ".part")) found = true;
+    }
+    if (e->tier.on) {                                   // count what is left (nothing, unless an unlink failed)
+        tier_enter(e, d, false, false);
+        if (partial) tier_enter(e, d, true, false);
+    }
+    return rc != DM_OK ? rc : found ? DM_OK : DM_ENOENT;
+}
+
+}  // namespace
+
+extern "C" {
+
+static int cache_remove_impl(dm_engine *e, const uint8_t *digests, uint32_t n, uint32_t flags, int32_t *status_out)
+{
+    if (!e || (n && (!digests || !status_out))) return fail(DM_EINVAL, "null argument");
+    if (flags & ~(DM_RM_ALIASES | DM_RM_PARTIAL)) return fail(DM_EINVAL, "unknown dm_cache_remove flag");
+    std::unordered_map<Digest, int32_t, DigestHash> seen;
+    std::string refused;                                // the first DM_ESTATE: what holds which digest
+    for (uint32_t i = 0; i < n; ++i) {
+        Digest d;
+        memcpy(d.b, digests + 32ull * i, 32);
+        auto ins = seen.emplace(d, DM_OK);
+        if (ins.second) {
+            std::string why;
+            ins.first->second = remove_one(e, d, (flags & DM_RM_PARTIAL) != 0, &why);
+            if (ins.first->second == DM_ESTATE && refused.empty()) refused = hex_of(d.b, 32) + " is held by " + why + ": retry later";
+            if (ins.first->second == DM_EIO) note_err(e, 0, fail(DM_EIO, why.c_str()));
+        }
+        status_out[i] = ins.first->second;
+    }
+    if ((flags & DM_RM_ALIASES) && n) {
+        std::lock_guard<std::mutex> g(e->alias_mu);
+        for (auto it = e->aliases.begin(); it != e->aliases.end();) {
+            auto k = seen.find(it->second);
+            if (k == seen.end() || k->second == DM_ESTATE) { ++it; continue; }
+            if (e->alias_log) fprintf(e->alias_log, "-\t%s\n", it->first.c_str());
+            it = e->aliases.erase(it);
+        }
+        if (e->alias_log) fflush(e->alias_log);
+    }
+    if (!refused.empty()) note_err(e, 0, fail(DM_ESTATE, refused.c_str()));
+    return DM_OK;
+}
+
 // ---- URL -> digest aliases -----------------------------------------------------------
 // The OnRequest hook (start.go:197-200) sees a URL.  OCI URLs name the digest; HuggingFace resolve/ URLs do
-// not, so a hit needs URL (or ETag) -> digest.  In memory: one hash map.  On the disk tier: an append-only
-// text log, one "<64 hex>\t<key>\n" per put, replayed at start (later lines win) and compacted when more
-// than half of it is dead.
+// not, so a hit needs URL (or ETag) -> digest.  In memory: one map ordered by key (dm_cache_alias_list pages it).  On
+// the disk tier: an append-only text log, one "<64 hex>\t<key>\n" per put and one "-\t<key>\n" tombstone per deletion,
+// replayed in order at start and compacted when more than half of it is dead.
 
 }  // extern "C"
 
@@ -590,11 +687,13 @@ void alias_load(dm_engine *e)
             Digest d;
             if (line.size() > 65 && line[64] == '\t' && digest_from_hex(line.c_str(), d.b) && alias_key_ok(line.c_str() + 65))
                 e->aliases[line.substr(65)] = d;                       // a torn last line simply fails these checks
+            else if (line.size() > 2 && line[0] == '-' && line[1] == '\t' && alias_key_ok(line.c_str() + 2))
+                e->aliases.erase(line.substr(2));                      // a tombstone (dm_cache_alias_del, DM_RM_ALIASES)
             line.clear();
         }
         fclose(f);
     }
-    if (lines > 2 * e->aliases.size() + 1024) {                        // mostly superseded entries: rewrite
+    if (lines > 2 * e->aliases.size() + 1024) {                        // mostly superseded or deleted entries: rewrite
         const std::string tmp = path + ".tmp";
         if (FILE *f = fopen(tmp.c_str(), "w")) {
             for (auto &kv : e->aliases) fprintf(f, "%s\t%s\n", hex_of(kv.second.b, 32).c_str(), kv.first.c_str());
@@ -634,6 +733,42 @@ int dm_cache_alias_get(dm_engine *e, const char *key, uint8_t digest_out[32])
     auto it = e->aliases.find(key);
     if (it == e->aliases.end()) return DM_ENOENT;
     memcpy(digest_out, it->second.b, 32);
+    return DM_OK;
+}
+
+static int cache_alias_del_impl(dm_engine *e, const char *key)
+{
+    if (!e || !key) return fail(DM_EINVAL, "null argument");
+    std::lock_guard<std::mutex> g(e->alias_mu);
+    auto it = e->aliases.find(key);
+    if (it == e->aliases.end()) return DM_ENOENT;
+    e->aliases.erase(it);
+    if (e->alias_log && !(fprintf(e->alias_log, "-\t%s\n", key) > 0 && fflush(e->alias_log) == 0))
+        return fail(DM_EIO, "could not append to aliases.log (the alias is deleted in memory only: it comes back at restart)");
+    return DM_OK;
+}
+
+static int cache_alias_list_impl(dm_engine *e, const char *prefix, const char *after, char *keys, size_t keys_cap,
+                                 uint8_t *digests_out, uint32_t cap, uint32_t *n_out, int *more)
+{
+    if (!e || !n_out || !more || (!keys && keys_cap) || (!digests_out && cap)) return fail(DM_EINVAL, "null argument");
+    *n_out = 0;
+    *more = 0;
+    const std::string pre = prefix ? prefix : "";
+    std::lock_guard<std::mutex> g(e->alias_mu);
+    auto it = e->aliases.lower_bound(pre);
+    if (after && pre.compare(after) <= 0) it = e->aliases.upper_bound(after);   // (an `after` below the prefix skips nothing)
+    size_t used = 0;
+    uint32_t k = 0;
+    for (; it != e->aliases.end() && it->first.compare(0, pre.size(), pre) == 0; ++it) {
+        const size_t len = it->first.size() + 1;
+        if (k == cap || used + len > keys_cap) { *more = 1; break; }
+        memcpy(keys + used, it->first.c_str(), len);
+        memcpy(digests_out + 32ull * k, it->second.b, 32);
+        used += len;
+        ++k;
+    }
+    *n_out = k;
     return DM_OK;
 }
 
@@ -684,6 +819,7 @@ int ingest_prepare(IngestBatch &B, uint32_t lo, uint32_t hi)
                 if (disk_safe && b->extents.size() == 1 && b->extents[0].len == want) {
                     B.ext[p] = b->extents[0];
                     b->extents.clear();
+                    b->parked = true;
                     B.parked[p] = it->second;
                 } else {
                     freed.insert(freed.end(), b->extents.begin(), b->extents.end());
@@ -972,6 +1108,16 @@ int dm_cache_meta(dm_engine *e, uint64_t reader, char *buf, size_t cap, size_t *
 int dm_cache_close(dm_engine *e, uint64_t reader) { return note_err(e, reader, cache_close_impl(e, reader)); }
 int dm_cache_follow(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size_hint) { return note_err(e, 0, cache_follow_impl(e, digest, reader, size_hint)); }
 int dm_cache_evict(dm_engine *e, const uint8_t digest[32]) { return note_err(e, 0, cache_evict_impl(e, digest)); }
+int dm_cache_remove(dm_engine *e, const uint8_t *digests, uint32_t n, uint32_t flags, int32_t *status_out)
+{
+    return note_err(e, 0, cache_remove_impl(e, digests, n, flags, status_out));
+}
+int dm_cache_alias_del(dm_engine *e, const char *key) { return note_err(e, 0, cache_alias_del_impl(e, key)); }
+int dm_cache_alias_list(dm_engine *e, const char *prefix, const char *after, char *keys, size_t keys_cap,
+                        uint8_t *digests_out, uint32_t cap, uint32_t *n_out, int *more)
+{
+    return note_err(e, 0, cache_alias_list_impl(e, prefix, after, keys, keys_cap, digests_out, cap, n_out, more));
+}
 int dm_cache_device_extents(dm_engine *e, uint64_t reader, void **dev_ptrs, uint64_t *lens, uint32_t max_ext) { return note_err(e, reader, cache_device_extents_impl(e, reader, dev_ptrs, lens, max_ext)); }
 int dm_ingest_device(dm_engine *e, const void *dev_base, const uint64_t *offsets, const uint64_t *lengths,
                      uint32_t n, const uint8_t *expect, uint8_t *digests_out, uint8_t *matched_out,

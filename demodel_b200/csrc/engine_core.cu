@@ -633,12 +633,14 @@ void unpark_many(dm_engine *e, std::vector<Parked> &verified, std::vector<Parked
             Blob *b = k.b.get();
             auto it = e->blobs.find(b->digest);
             if (it == e->blobs.end() || it->second.get() != b) { anew.push_back(Verified{b->digest, b->size, k.x}); continue; }
+            b->parked = false;
             if (b->in_hbm) { to_free.push_back(k.x); continue; }       // a stream re-homed it meanwhile: that copy wins
             b->extents.assign(1, k.x);
             b->in_hbm = true; lru_touch(e, b);
         }
         for (Parked &k : failed) {
             Blob *b = k.b.get();
+            b->parked = false;
             to_free.push_back(k.x);
             if (b->in_hbm || b->on_disk) continue;
             auto it = e->blobs.find(b->digest);
@@ -1207,7 +1209,7 @@ static void tier_erase(dm_engine *e, const Digest &d, bool saved)
 }
 
 // tier_mu held: (re)enter the files of `d` at their current st_size.
-static void tier_enter(dm_engine *e, const Digest &d, bool saved, bool use)
+void tier_enter(dm_engine *e, const Digest &d, bool saved, bool use)
 {
     DiskTier &T = e->tier;
     uint64_t bytes;
@@ -1525,10 +1527,20 @@ bool spill_one(dm_engine *e, Blob *b)
     if (fd < 0) return false;
     bool ok = d2h_to_fd(e, b->extents, b->size, fd);
     close(fd);
-    if (ok) ok = rename(tmp.c_str(), path.c_str()) == 0;
-    if (ok) write_sidecar(path + ".meta", *b);
-    else unlink(tmp.c_str());
-    return ok;
+    bool removed = false;                       // dm_cache_remove took the blob out meanwhile: its file must not appear
+    if (ok) {
+        std::lock_guard<std::mutex> g(e->mu);
+        removed = b->removed;
+        b->renaming = !removed;
+    }
+    if (ok && !removed) {
+        ok = rename(tmp.c_str(), path.c_str()) == 0;
+        if (ok) write_sidecar(path + ".meta", *b);
+        { std::lock_guard<std::mutex> g(e->mu); b->renaming = false; }
+        e->remove_cv.notify_all();
+    }
+    if (!ok || removed) unlink(tmp.c_str());
+    return ok && !removed;
 }
 
 void spill_main(dm_engine *e)
@@ -1555,12 +1567,14 @@ void spill_main(dm_engine *e)
         bool ok = have && tier_reserve(e, b->size + side.size(), false, &res) && spill_one(e, b.get());
         if (ok) tier_placed(e, b->digest, false, &res, true);
         else tier_release(e, res);
+        std::vector<Extent> gone;
         {
             std::lock_guard<std::mutex> g(e->mu);
-            if (have) b->readers--;
+            if (have) gone = reader_gone(b.get());
             b->on_disk = b->on_disk || ok;     // (a disk-backed publish or an import may have placed a copy meanwhile)
             b->spill_done = true;
         }
+        if (!gone.empty()) free_extents(e, gone);
         tier_unpin(e, b->digest, false, true);
         {
             std::lock_guard<std::mutex> g(e->spill_mu);
@@ -1843,6 +1857,29 @@ void drop_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, bool release_s
         auto it = e->inflight.find(sp->expect);
         if (it != e->inflight.end() && (it->second.expired() || it->second.lock() == sp)) e->inflight.erase(it);
     }
+    if (sp->held && erased) release_digest(e, sp->expect);
+}
+
+void hold_digest(dm_engine *e, const Digest &d, const char *what)
+{
+    std::lock_guard<std::mutex> g(e->mu);
+    auto &h = e->holds[d];
+    h.n++;
+    h.what = what;
+}
+
+void release_digest(dm_engine *e, const Digest &d)
+{
+    std::lock_guard<std::mutex> g(e->mu);
+    auto it = e->holds.find(d);
+    if (it != e->holds.end() && --it->second.n == 0) e->holds.erase(it);
+}
+
+std::vector<Extent> reader_gone(Blob *b)
+{
+    std::vector<Extent> ext;
+    if (--b->readers == 0 && b->removed) ext.swap(b->extents);
+    return ext;
 }
 
 int ensure_ingest_scratch(dm_engine *e, uint32_t n)

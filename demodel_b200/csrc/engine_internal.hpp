@@ -118,6 +118,10 @@ struct Blob {
     bool in_hbm = false;
     bool on_disk = false;
     bool spill_done = false;
+    // dm_cache_remove took it out of the index while readers had it open: the last dm_cache_close frees its extents
+    bool removed = false;
+    bool parked = false;                  // DM_ING_REPLACE is rewriting its extent (dm_cache_remove: DM_ESTATE)
+    bool renaming = false;                // a spill is moving its file into place: dm_cache_remove waits (remove_cv)
     std::vector<std::pair<std::string, std::string>> meta;   // response headers to replay on a hit
     std::string sidecar;                  // promoted from the disk tier (dm_cache_promote): its .meta text, replayed as is
 };
@@ -209,6 +213,7 @@ struct Stream {
     uint32_t pack_off = 0, pack_len = 0;
     std::vector<std::pair<std::string, std::string>> meta;   // dm_stream_set_meta
     bool load = false;         // the stream of a Load run by the loader threads: its completion wakes them (load_wake)
+    bool held = false;         // counted in e->holds under `expect` until drop_stream (dm_cache_remove: DM_ESTATE)
     uint32_t followers = 0;    // readers attached while the body is still arriving (request coalescing)
     uint32_t follow_reads = 0; // followers' copy-outs in flight: the extents must not be freed or handed over meanwhile
     bool completing = false;   // digest known, extents being handed to the index: followers wait for Done
@@ -380,6 +385,11 @@ struct dm_engine {
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp
     std::unordered_map<Digest, std::weak_ptr<Stream>, DigestHash> inflight;   // open streams by expected digest
+    // Digests something is placing or loading outside e->loads: open streams that expect them, and running
+    // dm_cache_promote / verify / import / dm_stream_resume_saved calls.  dm_cache_remove refuses them (DM_ESTATE).
+    struct Hold { uint32_t n = 0; const char *what = ""; };
+    std::unordered_map<Digest, Hold, DigestHash> holds;
+    std::condition_variable remove_cv;  // (with mu) a spill finished moving a blob's file into place (Blob::renaming)
     std::mutex reader_mu[kStripes];
     std::unordered_map<uint64_t, std::shared_ptr<Reader>> readers[kStripes];
     Blob *lru_head = nullptr, *lru_tail = nullptr;   // HBM-resident blobs, least recently used first (guarded by mu):
@@ -473,7 +483,8 @@ struct dm_engine {
     std::atomic<uint64_t> st_packed{0}, st_packs{0};
 
     std::mutex alias_mu;             // URL / ETag -> digest (dm_cache_alias_put/get); log = <cas_dir>/aliases.log
-    std::unordered_map<std::string, Digest> aliases;
+    // ordered by key: dm_cache_alias_list pages from a prefix or a key in O(log n) instead of sorting every page
+    std::map<std::string, Digest> aliases;
     FILE *alias_log = nullptr;
     std::atomic<uint64_t> n_suspended{0};   // *.ckpt under <cas_dir>/partial
 
@@ -575,6 +586,17 @@ std::shared_ptr<Stream> find_stream(dm_engine *e, uint64_t id);
 void drop_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, bool release_slot);
 int ensure_ingest_scratch(dm_engine *e, uint32_t n);
 void alias_load(dm_engine *e);                // dm_engine_create: replay <cas_dir>/aliases.log
+// e->holds (dm_cache_remove refuses a held digest).  `what` is a string literal: it names the holder in the refusal.
+void hold_digest(dm_engine *e, const Digest &d, const char *what);
+void release_digest(dm_engine *e, const Digest &d);
+struct DigestHold {                           // hold_digest for the lifetime of a call
+    dm_engine *e; Digest d;
+    DigestHold(dm_engine *e_, const Digest &d_, const char *what) : e(e_), d(d_) { hold_digest(e, d, what); }
+    ~DigestHold() { release_digest(e, d); }
+};
+// e->mu held: one reader fewer on a blob; returns the extents to free (outside the lock) when it was the last reader of
+// a blob dm_cache_remove took out of the index
+std::vector<Extent> reader_gone(Blob *b);
 bool digest_from_hex(const char *hex, uint8_t out[32]);
 bool alias_key_ok(const char *key);           // 1..4096 bytes without control characters: one line of aliases.log
 void sweep_incoming(const std::string &dir);  // remove files under incoming/ of processes that are gone
@@ -610,5 +632,6 @@ void tier_unstage(dm_engine *e, const std::string &path);
 bool tier_stage_to_blob(dm_engine *e, const std::string &path, uint64_t size, uint64_t side, TierRes *r);
 void tier_build(dm_engine *e);                         // tier_mu held: the walk that builds the index
 bool tier_make_room(dm_engine *e, uint64_t need, bool partial);   // tier_mu held: evict until `need` more bytes fit
+void tier_enter(dm_engine *e, const Digest &d, bool saved, bool use);   // tier_mu held, limit on: count the files of d as they are now
 
 }  // namespace dmi

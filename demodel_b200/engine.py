@@ -10,13 +10,13 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Iterable, Optional, Sequence
+from typing import Iterable, Iterator, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
 from ._lib import (DM_ENOENT, DM_IMP_LINK, DM_ING_FORCE_DEEP, DM_ING_FORCE_WIDE, DM_ING_HASH_ONLY, DM_ING_REPLACE,
-                   DM_OK, DmConfig, DmError, DmStats, check)
+                   DM_OK, DM_RM_ALIASES, DM_RM_PARTIAL, DmConfig, DmError, DmStats, check)
 
 
 def _buf_ptr(buf) -> tuple[C.c_void_p, int]:
@@ -253,6 +253,21 @@ class Engine:
         check(rc, "dm_cache_evict")
         return True
 
+    def cache_remove(self, digests: Sequence[bytes], aliases: bool = False, partial: bool = False) -> list[int]:
+        """dm_cache_remove: delete blobs from both tiers.  aliases=True also deletes every alias naming a removed
+        digest; partial=True also deletes a download of it saved by dm_stream_suspend.  One status per digest: DM_OK,
+        DM_ENOENT (on neither tier), DM_ESTATE (being placed or loaded right now, nothing removed: retry later;
+        error_detail(0) says what holds it) or DM_EIO."""
+        digests = list(digests)
+        if any(len(d) != 32 for d in digests):
+            raise ValueError("every digest must be 32 bytes")
+        status = (C.c_int32 * max(len(digests), 1))()
+        blob = b"".join(digests)
+        flags = (DM_RM_ALIASES if aliases else 0) | (DM_RM_PARTIAL if partial else 0)
+        check(self._lib.dm_cache_remove(self._h, C.cast(C.c_char_p(blob), C.c_void_p) if digests else None,
+                                        len(digests), flags, status), "dm_cache_remove")
+        return list(status[:len(digests)])
+
     def promote(self, digests: Sequence[bytes]) -> list[int]:
         """dm_cache_promote: bring cached blobs back into HBM, each disk copy verified on the GPU as it loads.
         One status per digest: DM_OK (in HBM now), DM_ENOENT, DM_ENOMEM, DM_EIO, DM_ECUDA or DM_ECORRUPT (the disk
@@ -342,6 +357,36 @@ class Engine:
             return None
         check(rc, "dm_cache_alias_get")
         return bytes(out)
+
+    def alias_del(self, key: str) -> bool:
+        """dm_cache_alias_del: False when the key was not known."""
+        rc = self._lib.dm_cache_alias_del(self._h, key.encode())
+        if rc == DM_ENOENT:
+            return False
+        check(rc, "dm_cache_alias_del")
+        return True
+
+    def alias_list(self, prefix: str = "", page: int = 1024, keys_bytes: int = 1 << 20) -> Iterator[tuple[str, bytes]]:
+        """dm_cache_alias_list, paged: every (key, digest) whose key starts with `prefix`, in ascending byte order of
+        the UTF-8 keys.  Each page asks for up to `page` entries in a `keys_bytes` key buffer (a key of up to 4096
+        bytes always fits)."""
+        if page < 1 or keys_bytes < 4097:
+            raise ValueError("page must be >= 1 and keys_bytes >= 4097")
+        keys = (C.c_char * keys_bytes)()
+        digs = (C.c_uint8 * (32 * page))()
+        n, more = C.c_uint32(), C.c_int()
+        after = None
+        while True:
+            check(self._lib.dm_cache_alias_list(self._h, prefix.encode(), after, keys, keys_bytes, digs, page,
+                                                C.byref(n), C.byref(more)), "dm_cache_alias_list")
+            raw, d, pos = keys.raw, bytes(digs), 0
+            for i in range(n.value):
+                end = raw.index(b"\0", pos)
+                after = raw[pos:end]
+                yield after.decode(), d[32 * i:32 * i + 32]
+                pos = end + 1
+            if not more.value:
+                return
 
     def proxy_fetch(self, url: str, body, expect: Optional[bytes] = None, chunk: int = 32768) -> tuple[bytes, bool]:
         """OnResponse twin for one body fetched under `url` (BodyTee + SetURL): (digest, matched)."""

@@ -646,6 +646,133 @@ func (p *Pool) List(after *[32]byte, limit int) ([][32]byte, []uint64, error) {
 	return digests, sizes, nil
 }
 
+// Remove deletes blobs from the cache (dm_cache_remove) on the engine that owns each digest, the engines in
+// parallel.  aliases also deletes every alias naming a removed digest on that engine; partial also deletes a download
+// of it saved by Suspend.  It blocks until every blob has a status: 0 (DM_OK) or a negative dm_err - DM_ENOENT (on
+// neither tier), DM_ESTATE (something is placing or loading it right now and nothing of it was removed: retry later)
+// or DM_EIO.  Open HitReaders keep reading what they opened.  Aliases of a blob imported without a known digest live
+// on engine 0 (see Import): delete those with AliasDel.
+func (p *Pool) Remove(digests [][32]byte, aliases, partial bool) ([]int, error) {
+	status := make([]int, len(digests))
+	byEngine := make(map[*C.dm_engine][]int)
+	for i := range digests {
+		e := p.engineFor(&digests[i])
+		byEngine[e] = append(byEngine[e], i)
+	}
+	var flags C.uint32_t
+	if aliases {
+		flags |= C.DM_RM_ALIASES
+	}
+	if partial {
+		flags |= C.DM_RM_PARTIAL
+	}
+	errs := make(chan error, len(byEngine))
+	for e, idx := range byEngine {
+		go func(e *C.dm_engine, idx []int) {
+			buf := make([][32]byte, len(idx))
+			for k, i := range idx {
+				buf[k] = digests[i]
+			}
+			st := make([]C.int32_t, len(idx))
+			err := check(e, 0, C.dm_cache_remove(e, (*C.uint8_t)(unsafe.Pointer(&buf[0][0])), C.uint32_t(len(idx)), flags, &st[0]))
+			for k, i := range idx {
+				status[i] = int(st[k])
+			}
+			errs <- err
+		}(e, idx)
+	}
+	var first error
+	for range byEngine {
+		if err := <-errs; err != nil && first == nil {
+			first = err
+		}
+	}
+	return status, first
+}
+
+// AliasDel deletes an alias (dm_cache_alias_del) on every engine: an alias lives on the engine that verified its
+// body, and Import puts the aliases of files of unknown digest on engine 0.  It reports whether any engine had it.
+func (p *Pool) AliasDel(key string) (bool, error) {
+	ck := C.CString(key)
+	defer C.free(unsafe.Pointer(ck))
+	found := false
+	for _, e := range p.engines {
+		rc := C.dm_cache_alias_del(e, ck)
+		if rc == C.DM_OK {
+			found = true
+		} else if rc != C.DM_ENOENT {
+			return found, check(e, 0, rc)
+		}
+	}
+	return found, nil
+}
+
+// Alias is one entry of AliasList.
+type Alias struct {
+	Key    string
+	Digest [32]byte
+}
+
+// AliasList returns up to limit aliases whose keys start with prefix, strictly after `after` ("" for the start),
+// merged across the engines in ascending byte order of the keys (dm_cache_alias_list).  Fewer than limit entries
+// means the listing is complete; the next page starts after the last key returned.  A key present on two engines is
+// listed once, with the digest of the lowest-numbered engine.
+func (p *Pool) AliasList(prefix, after string, limit int) ([]Alias, error) {
+	if limit <= 0 {
+		return nil, nil
+	}
+	cp := C.CString(prefix)
+	defer C.free(unsafe.Pointer(cp))
+	var ca *C.char
+	if after != "" {
+		ca = C.CString(after)
+		defer C.free(unsafe.Pointer(ca))
+	}
+	const keyBytes = 1 << 20 // a key is at most 4096 bytes, so every page holds at least one
+	keys := (*[keyBytes]byte)(C.malloc(keyBytes))
+	defer C.free(unsafe.Pointer(keys))
+	var all []Alias
+	seen := make(map[string]bool)
+	for _, e := range p.engines {
+		digs := make([][32]byte, limit)
+		from := ca
+		for got := 0; got < limit; {
+			var n C.uint32_t
+			var more C.int
+			if err := check(e, 0, C.dm_cache_alias_list(e, cp, from, (*C.char)(unsafe.Pointer(&keys[0])), keyBytes,
+				(*C.uint8_t)(unsafe.Pointer(&digs[0][0])), C.uint32_t(limit-got), &n, &more)); err != nil {
+				return nil, err
+			}
+			pos, last := 0, ""
+			for k := 0; k < int(n); k++ {
+				end := bytes.IndexByte(keys[pos:], 0) + pos
+				last = string(keys[pos:end])
+				if !seen[last] {
+					seen[last] = true
+					all = append(all, Alias{last, digs[k]})
+				}
+				pos = end + 1
+			}
+			got += int(n)
+			if more == 0 || n == 0 {
+				break
+			}
+			if from != ca {
+				C.free(unsafe.Pointer(from))
+			}
+			from = C.CString(last)
+		}
+		if from != ca {
+			C.free(unsafe.Pointer(from))
+		}
+	}
+	sort.Slice(all, func(a, b int) bool { return all[a].Key < all[b].Key })
+	if len(all) > limit {
+		all = all[:limit]
+	}
+	return all, nil
+}
+
 // ---- requests are URLs, not digests (start.go:197-200) ------------------------------------------------------
 
 // SetURL records the request URL with the body: it goes into the sidecar, and once the body has verified the

@@ -268,6 +268,40 @@ int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t
 int dm_cache_meta(dm_engine *e, uint64_t reader, char *buf, size_t cap, size_t *len);
 int dm_cache_close(dm_engine *e, uint64_t reader);
 int dm_cache_evict(dm_engine *e, const uint8_t digest[32]);   /* HBM tier only; disk copy stays */
+/* dm_cache_remove flags */
+#define DM_RM_ALIASES 0x1u   /* also delete every alias whose digest is removed (logged as tombstones, see the aliases) */
+#define DM_RM_PARTIAL 0x2u   /* also delete a download of the digest saved by dm_stream_suspend */
+/* Remove blobs from the cache on request: the operator's delete (a model nobody uses, a superseded revision, a
+ * repository that must stop being served, a bad upload).  Blocks until every status is known; duplicates in digests[]
+ * are handled once.  status_out[i]:
+ *   DM_OK        removed from every tier that held it (rules below)
+ *   DM_ENOENT    on neither tier, and no saved download under DM_RM_PARTIAL (its aliases still go under DM_RM_ALIASES)
+ *   DM_ESTATE    something is placing or loading the digest right now, and nothing of it is removed: retry later.
+ *                dm_error_detail(e, 0) names the first such digest and what holds it: a stream opened with it as its
+ *                expected digest (HBM, verify-only or disk-backed, until dm_stream_finish / dm_stream_abort returns), a
+ *                running load (dm_cache_open_verified, dm_cache_promote), a running dm_cache_verify or dm_cache_import
+ *                that holds it, a DM_ING_REPLACE re-ingest of it in a running dm_ingest_device, or a
+ *                dm_stream_resume_saved taking its saved download over
+ *   DM_EIO       an unlink failed with something other than ENOENT: what was already removed stays removed, and the
+ *                engine's indexes (HBM, disk-tier limit) match what is left on disk; dm_error_detail(e, 0) says which
+ * HBM copy: leaves the index and the LRU order at once, so dm_cache_contains, dm_cache_open, dm_cache_open_verified,
+ * dm_cache_follow and dm_cache_promote miss from then on.  Readers that have it open keep reading the same extent until
+ * dm_cache_close (dm_cache_device_extents on them stays valid); the extent is freed, and hbm_cas_used drops, when the
+ * last of them closes.  (dm_cache_evict instead refuses while readers are open.)  A queued spill of the blob is
+ * dropped; a running one finishes its .part and unlinks it instead of renaming it into place: no file of the digest
+ * appears under blobs/ after DM_OK.
+ * Disk copy: the blob file is unlinked, then its sidecar.  Readers that hold a descriptor (dm_cache_open, a follower of
+ * a completed disk-backed body) keep reading it.  With a disk-tier limit, used_bytes falls by the file and its sidecar;
+ * evicted_files, evicted_bytes and refused do not move (a removal is not an eviction).
+ * DM_RM_PARTIAL: <hex>.ckpt, then <hex>.part under partial/ are unlinked; dm_stream_resume_saved is DM_ENOENT for the
+ * digest afterwards and dm_stats.suspended drops.
+ * Not a ban: a new download, an import, a promotion of a re-imported file or dm_ingest_device may cache the digest
+ * again, as may a stream opened without an expected digest whose bytes hash to it.  blobs_committed,
+ * blobs_mismatched and the byte counters do not move.
+ * Returns DM_OK once every status is filled; DM_EINVAL on bad arguments or unknown flags.  Without cas_dir only the
+ * HBM tier is looked at (DM_RM_PARTIAL finds nothing).  One digest at a time holds the disk tier's lock (see
+ * dm_cache_set_disk_limit) for its unlinks. */
+int dm_cache_remove(dm_engine *e, const uint8_t *digests, uint32_t n, uint32_t flags, int32_t *status_out);
 /* Bring cached blobs back into HBM, verifying each disk copy on the GPU as it loads.  A blob leaves HBM when it is
  * evicted or the engine restarts, and dm_cache_open serves it from <cas_dir>/blobs/ from then on, unverified and
  * without dm_cache_device_extents (dm_cache_open_verified loads it the same way on a hit).  This reads each file into the pinned ring, DMAs it into a fresh HBM extent and
@@ -465,9 +499,21 @@ int dm_cache_follow(dm_engine *e, const uint8_t digest[32], uint64_t *reader, ui
  * NUL-terminated string up to 4096 bytes.  With cas_dir the index is an append-only log
  * (<cas_dir>/aliases.log) replayed by dm_engine_create; a put for an existing key replaces it.
  * dm_cache_alias_get: DM_ENOENT when the key is unknown (the digest may since have been evicted from both
- * tiers: dm_cache_open decides). */
+ * tiers: dm_cache_open decides).
+ * dm_cache_alias_del: DM_OK, or DM_ENOENT when the key is unknown.  A deletion (and each alias DM_RM_ALIASES deletes)
+ * is appended to the log as a tombstone line "-\t<key>", and replay applies the lines in order.  Tombstones and the
+ * lines they deleted count as dead when the log is compacted at start.  An engine of an older build skips tombstone
+ * lines as unreadable, so a deleted alias comes back if the cache is downgraded.
+ * dm_cache_alias_list: keys starting with `prefix` ("" or NULL = all), in ascending byte order, strictly after `after`
+ * (NULL = from the start).  Keys are copied NUL-terminated back to back into keys[keys_cap]; digests_out[i] is key i's
+ * digest.  Stops at cap entries or when the next key does not fit; *more = 1 if anything was left out.  Stateless,
+ * like dm_cache_list: page by passing the last key returned.  The index is ordered by key, so a page costs
+ * O(log n + page) at any number of aliases. */
 int dm_cache_alias_put(dm_engine *e, const char *key, const uint8_t digest[32]);
 int dm_cache_alias_get(dm_engine *e, const char *key, uint8_t digest_out[32]);
+int dm_cache_alias_del(dm_engine *e, const char *key);
+int dm_cache_alias_list(dm_engine *e, const char *prefix, const char *after, char *keys, size_t keys_cap,
+                        uint8_t *digests_out, uint32_t cap, uint32_t *n_out, int *more);
 
 /* ---- device-resident ingest -------------------------------------------- */
 /* Hash-and-cache n blobs whose bytes are ALREADY in this GPU's HBM (landed
