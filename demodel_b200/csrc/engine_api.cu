@@ -1671,8 +1671,10 @@ bool blob_in_hbm(dm_engine *e, const Digest &d)
 
 // Open the check of the file `fd` at `path` (c.seen is its fstat).  The stream takes over fd, or it is closed here.
 // Returns 1 with c.stream open (a disk-backed check already finishing, a tiny one waiting for its flush) or c's final
-// status.
-int check_open(dm_engine *e, Check &c, int fd, const std::string &path)
+// status.  `ring`: the check is a ring load (dm_cache_open_verified_ring), always read back through ring slabs, never
+// packed; it takes over the caller's hold on c.d (released when it is dropped), and *out is its stream.
+int check_open(dm_engine *e, Check &c, int fd, const std::string &path, std::unique_ptr<RingLoad> ring = nullptr,
+               std::shared_ptr<Stream> *out = nullptr)
 {
     const uint64_t size = (uint64_t)c.seen.st_size;
     auto sp = std::make_shared<Stream>();
@@ -1680,7 +1682,7 @@ int check_open(dm_engine *e, Check &c, int fd, const std::string &path)
     if (c.known) sp->expect = c.d;
     sp->check_only = sp->verify_only = true;
     sp->size_hint = size;
-    c.tiny = e->tiny_max && size <= e->tiny_max;
+    c.tiny = !ring && e->tiny_max && size <= e->tiny_max;
     if (c.tiny) {
         sp->small.reset(new uint8_t[std::max<uint64_t>(size, 1)]);
         sp->small_cap = (uint32_t)size;
@@ -1712,12 +1714,14 @@ int check_open(dm_engine *e, Check &c, int fd, const std::string &path)
         e->free_slots.pop_back();
     }
     sp->id = e->next_id.fetch_add(1);
+    if (ring) { sp->ring = std::move(ring); sp->held = true; }
     {
         const int k = (int)(sp->id % kStripes);
         std::lock_guard<std::mutex> g(e->stripe_mu[k]);
         e->streams[k][sp->id] = sp;
         e->n_streams++;
     }
+    if (out) *out = sp;
     if (!c.tiny) {                                       // flushed straight away: every byte is already in the file
         std::lock_guard<std::mutex> g(sp->mu);
         sp->st = St::Finishing;
@@ -1751,7 +1755,8 @@ int check_verdict(dm_engine *e, Check &c)
 // What dm_cache_verify and dm_cache_import share: the ring's device mirror (read-backs, and a tiny check that finds
 // no pack, stage slabs there), a slot budget drawn from the reservation dm_cache_promote uses, and kVerifyThreads
 // threads that open checks and collect their verdicts.  The live proxy keeps its ring: at most a quarter of the slabs'
-// worth of disk-backed checks are open at once, and each holds at most two slabs.
+// worth of disk-backed checks are open at once, and each holds at most two slabs.  Ring loads (below) have a quarter of
+// their own, so checks and ring loads together never hold more than half of the ring.
 class CheckRun {
 public:
     CheckRun(dm_engine *e, size_t n_work) : e_(e)
@@ -1873,6 +1878,102 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
     return DM_OK;
 }
+
+// ---- ring loads (dm_cache_open_verified_ring) -------------------------------------------------------------------
+// A check of a tier file (above) whose read-back slabs also serve one reader (struct RingLoad).  Each load holds at
+// most kRingLoadSlabs slabs: the two of the hash side (disk_feed) and two that the reader may still be copying from.
+// All ring loads together hold at most a quarter of the ring's slabs (their own quarter: checks have another), and each
+// takes one slot of the reservation dm_cache_promote, dm_cache_verify and dm_cache_import share.
+
+}  // extern "C"
+
+namespace dmi {
+
+constexpr uint32_t kRingLoadSlabs = 4;
+
+int ring_load_open(dm_engine *e, const Digest &d, std::shared_ptr<Stream> *out, uint64_t *size, std::string *side)
+{
+    const size_t share = std::max<size_t>(1, e->slab_store.size() / 4);
+    const uint32_t cap = (uint32_t)std::min<size_t>(kRingLoadSlabs, share);
+    {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        const size_t free = e->free_slots.size();
+        if (free <= e->promote_reserved || (free - e->promote_reserved) / 2 < 1)
+            return fail(DM_ENOMEM, "no stream slot to spare for a ring load");
+        if (e->ring_load_slabs + cap > share)
+            return fail(DM_ENOMEM, "the ring slabs ring loads may hold are all taken: retry later, or serve the blob with dm_cache_open");
+        e->promote_reserved++;
+        e->ring_load_slabs += cap;
+    }
+    auto unreserve = [&] {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        e->promote_reserved--;
+        e->ring_load_slabs -= cap;
+    };
+    if (const int rc = ensure_dev_ring(e); rc != DM_OK) { unreserve(); return rc; }
+    hold_digest(e, d, "a running ring load (dm_cache_open_verified_ring)");
+    Check c;
+    c.d = d;
+    int fd = -1;
+    int rc = open_disk_copy(e, d, &fd, &c.seen, side);
+    if (rc == DM_OK) {
+        auto R = std::make_unique<RingLoad>();
+        R->cap = cap;
+        R->seen = c.seen;
+        rc = check_open(e, c, fd, blob_path(e, d.b), std::move(R), out);
+    }
+    if (rc != 1) { release_digest(e, d); unreserve(); return rc; }
+    *size = (uint64_t)c.seen.st_size;
+    return DM_OK;
+}
+
+void ring_load_settle(dm_engine *e, const std::shared_ptr<Stream> &sp)
+{
+    Stream *s = sp.get();
+    RingLoad *R = s->ring.get();
+    int status;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        status = s->cuda_failed ? DM_ECUDA : s->lost != DM_OK ? s->lost : s->matched ? DM_OK : DM_ECORRUPT;
+    }
+    if (status == DM_OK) tier_touch(e, s->expect);              // a use of the blob, as a verified open is
+    else if (status == DM_ECORRUPT) drop_corrupt(e, s->expect, R->seen);
+    drop_stream(e, sp, true);                                   // its slot, and its hold on the digest
+    bool unreserve;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        unreserve = R->slot_reserved;
+        R->slot_reserved = false;
+        R->status = status;
+        R->settled = true;
+    }
+    if (unreserve) { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved--; }
+    s->cv.notify_all();
+}
+
+void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp)
+{
+    Stream *s = sp.get();
+    RingLoad *R = s->ring.get();
+    bool stop, unreserve;
+    {
+        std::lock_guard<std::mutex> g(s->mu);
+        R->closed = true;
+        ring_release(e, sp);
+        stop = !R->settled && s->st != St::Done && s->st != St::Aborted;
+        unreserve = R->slot_reserved;
+        R->slot_reserved = false;
+    }
+    // slabs still staged come back from the abort, those being hashed when their jobs are reaped (R->closed)
+    if (stop) stream_abort_impl(e, s->id);
+    std::lock_guard<std::mutex> g(e->slot_mu);
+    if (unreserve) e->promote_reserved--;
+    e->ring_load_slabs -= R->cap;
+}
+
+}  // namespace dmi
+
+extern "C" {
 
 // ---- importing files from outside the cache (dm_cache_import) ---------------------------------------------------
 // Each source is first copied (or hard-linked) to a private file under <cas_dir>/incoming/.  That file is checked the

@@ -125,6 +125,42 @@ static int cache_open_verified_impl(dm_engine *e, const uint8_t digest[32], uint
     return DM_OK;
 }
 
+// A blob in HBM opens as with dm_cache_open.  One on the disk tier only gets a ring load of its own (struct RingLoad):
+// the reader is served from the ring slabs that carry the file to the kernel, and no HBM extent is taken.
+static int cache_open_verified_ring_impl(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size)
+{
+    if (!e || !digest || !reader) return fail(DM_EINVAL, "null argument");
+    Digest d;
+    memcpy(d.b, digest, 32);
+    auto r = std::make_shared<Reader>();
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(d);
+        if (it != e->blobs.end() && it->second->in_hbm) {      // verified when it entered HBM: an ordinary hit
+            r->blob = it->second;
+            r->blob->readers++;
+            lru_touch(e, r->blob.get());
+            r->size = r->blob->size;
+        }
+    }
+    if (!r->blob) {
+        if (e->cas_dir.empty()) return DM_ENOENT;
+        tier_pin(e, d);                                  // the load's, then the reader's until dm_cache_close
+        const int rc = ring_load_open(e, d, &r->ring, &r->size, &r->disk_meta);
+        if (rc != DM_OK) { tier_unpin(e, d); return rc; }
+        r->disk_digest = d;
+        r->disk_pin = true;
+    }
+    const uint64_t id = e->next_id.fetch_add(1);
+    {
+        std::lock_guard<std::mutex> g(e->reader_mu[id % kStripes]);
+        e->readers[id % kStripes][id] = r;
+    }
+    *reader = id;
+    if (size) *size = r->size;
+    return DM_OK;
+}
+
 static std::shared_ptr<Reader> find_reader(dm_engine *e, uint64_t id)
 {
     std::lock_guard<std::mutex> g(e->reader_mu[id % kStripes]);
@@ -298,6 +334,57 @@ static int follow_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t 
     return DM_OK;
 }
 
+// A read of a ring load's reader (dm_cache_open_verified_ring), forward only.  Waits until the slab holding `off` has been
+// read back, then copies out of it and out of the slabs after it that are already there.  Byte size - 1 and the EOF
+// read wait for the verdict; once it has failed, every read returns its status.
+static int ring_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t len, size_t *nread)
+{
+    std::lock_guard<std::mutex> gr(r->mu);
+    Stream *s = r->ring.get();
+    RingLoad *R = s->ring.get();
+    if (off > r->size) return fail(DM_ERANGE, "offset beyond blob end");
+    len = (size_t)std::min<uint64_t>(len, r->size - off);
+    const uint64_t gate = r->size ? r->size - 1 : 0;     // bytes from here on wait for the verdict
+    std::unique_lock<std::mutex> g(s->mu);
+    if (R->started && off < R->next)
+        return fail(DM_ESTATE, "a dm_cache_open_verified_ring reader reads forward only: this read starts below the end of the previous one");
+    R->started = true;
+    R->next = off;
+    if (off > R->need) { R->need = off; ring_release(e, r->ring); disk_feed(e, r->ring); }
+    auto slab_at = [&](uint64_t at) -> const RingLoad::Held * {
+        for (const RingLoad::Held &h : R->held) if (at >= h.off && at < h.off + h.n) return &h;
+        return nullptr;
+    };
+    s->cv.wait(g, [&] { return R->settled || (len == 0 && off < r->size) || (off < gate && slab_at(off)); });
+    if (R->settled && R->status != DM_OK)
+        return fail(R->status, R->status == DM_ECORRUPT ? "the disk tier file does not hash to its digest: file and sidecar removed"
+                             : R->status == DM_EIO ? "the disk tier file could not be read" : "a CUDA copy or launch failed while the blob was hashed");
+    uint8_t *out = static_cast<uint8_t *>(buf);
+    size_t done = 0;
+    while (done < len) {
+        const uint64_t at = off + done;
+        const uint64_t limit = R->settled ? r->size : gate;
+        const RingLoad::Held *h = at < limit ? slab_at(at) : nullptr;
+        if (!h) break;
+        const size_t n = (size_t)std::min<uint64_t>(len - done, std::min<uint64_t>(h->off + h->n, limit) - at);
+        const uint8_t *src = h->slab->host + (at - h->off);
+        // the slab stays out of the ring while this copy runs: `need` is at most `at`, and only this reader moves it
+        g.unlock();
+        memcpy(out + done, src, n);
+        g.lock();
+        done += n;
+        R->next = R->need = off + done;
+        ring_release(e, r->ring);
+        disk_feed(e, r->ring);
+    }
+    if (done == 0 && len && R->settled)
+        return fail(DM_ESTATE, "the ring load no longer holds the bytes at this offset");
+    g.unlock();
+    e->st_served += done;
+    if (nread) *nread = done;
+    return DM_OK;
+}
+
 // Start the D2H of [start, start + <=4 MiB) of the blob into a read-ahead window.
 static cudaError_t window_fill(dm_engine *e, Reader *r, Window &w, uint64_t start)
 {
@@ -324,6 +411,7 @@ static int cache_read_impl(dm_engine *e, uint64_t reader, uint64_t off, void *bu
     std::shared_ptr<Reader> r = find_reader(e, reader);
     if (!r) return fail(DM_EINVAL, "unknown reader id");
     if (nread) *nread = 0;
+    if (r->ring) return ring_read(e, r.get(), off, buf, len, nread);
     if (r->follow) {
         int rc = follow_read(e, r.get(), off, buf, len, nread);
         if (rc != 1) return rc;                 // 1: the body completed and was published: fall through to the blob
@@ -458,6 +546,10 @@ static int cache_close_impl(dm_engine *e, uint64_t reader)
         }
         if (!gone.empty()) free_extents(e, gone);
     }
+    if (r->ring) {
+        { std::lock_guard<std::mutex> g(r->mu); ring_load_close(e, r->ring); }
+        tier_unpin(e, r->disk_digest);
+    }
     if (r->fd >= 0) {
         close(r->fd);
         if (r->disk_pin) tier_unpin(e, r->disk_digest);
@@ -535,6 +627,7 @@ static int cache_device_extents_impl(dm_engine *e, uint64_t reader, void **dev_p
     std::shared_ptr<Reader> r = find_reader(e, reader);
     if (!r) return fail(DM_EINVAL, "unknown reader id");
     if (!r->blob && r->load) return fail(DM_ESTATE, "the blob is still being loaded and verified: read it to its end first");
+    if (r->ring) return fail(DM_ESTATE, "a ring load's reader has no device extents (dm_cache_open_verified_ring)");
     if (!r->blob) return fail(DM_ESTATE, "blob is on the disk tier only");
     const auto &ext = r->blob->extents;
     uint64_t left = r->blob->size;
@@ -1103,6 +1196,7 @@ int dm_synth_fill_device_many(dm_engine *e, uint64_t seed, uint64_t first_blob, 
 // ---- exported wrappers: file the error text under the reader id (dm_error_detail) ----
 int dm_cache_open(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_impl(e, digest, reader, size)); }
 int dm_cache_open_verified(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_verified_impl(e, digest, reader, size)); }
+int dm_cache_open_verified_ring(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_verified_ring_impl(e, digest, reader, size)); }
 int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t len, size_t *nread) { return note_err(e, reader, cache_read_impl(e, reader, off, buf, len, nread)); }
 int dm_cache_meta(dm_engine *e, uint64_t reader, char *buf, size_t cap, size_t *len) { return note_err(e, reader, cache_meta_impl(e, reader, buf, cap, len)); }
 int dm_cache_close(dm_engine *e, uint64_t reader) { return note_err(e, reader, cache_close_impl(e, reader)); }

@@ -719,6 +719,29 @@ void completer_main(dm_engine *e)
     }
 }
 
+// A ring load's slab whose job has been reaped: it no longer comes back by itself (slabs_returning), and goes back to
+// the ring now or once its reader is done with it.  Stream mutex held.
+static void ring_reaped(dm_engine *e, const std::shared_ptr<Stream> &sp, Slab *slab)
+{
+    e->slabs_returning.fetch_sub(1, std::memory_order_relaxed);
+    bool found = false;
+    for (RingLoad::Held &h : sp->ring->held)
+        if (h.slab == slab) { h.reaped = found = true; break; }
+    if (!found) slab_put(e, slab);              // (not kept: cannot happen, but never lose a slab)
+    ring_release(e, sp);
+}
+
+void ring_release(dm_engine *e, const std::shared_ptr<Stream> &sp)
+{
+    RingLoad *R = sp->ring.get();
+    for (auto it = R->held.begin(); it != R->held.end();) {
+        if (it->reaped && (R->closed || (R->started && it->off + it->n <= R->need))) {
+            slab_put(e, it->slab);
+            it = R->held.erase(it);
+        } else ++it;
+    }
+}
+
 void reap_cycle(dm_engine *e, Cycle &c)
 {
     std::vector<dm_engine::DoneItem> finished;          // handed to the completion threads under ONE lock at the end
@@ -729,8 +752,8 @@ void reap_cycle(dm_engine *e, Cycle &c)
         e->st_kernel_ms += ms;
     }
     e->st_hashed += c.bytes;
-    for (Slab *sl : c.job_slabs) if (sl) slab_return(e, sl);
-    c.job_slabs.clear();
+    // (a ring load's slab may still be wanted by its reader: see ring_reaped below)
+    for (size_t i = 0; i < c.job_slabs.size(); ++i) if (c.job_slabs[i] && !c.streams[i]->ring) slab_return(e, c.job_slabs[i]);
     for (size_t i = 0; i < c.streams.size(); ++i) {
         std::shared_ptr<Stream> &sp = c.streams[i];
         bool free_now = false, wake = false;
@@ -743,6 +766,7 @@ void reap_cycle(dm_engine *e, Cycle &c)
                 pack_release_member(e, sp.get());
             }
             sp->jobs_inflight--;
+            if (sp->ring && c.job_slabs[i]) ring_reaped(e, sp, c.job_slabs[i]);
             if (sp->disk) disk_feed(e, sp);                        // a staged slab was used up: read the next one back
             free_now = sp->st == St::Aborted && sp->jobs_inflight == 0;
             wake = sp->ckpt_waiter;
@@ -770,7 +794,7 @@ void reap_cycle(dm_engine *e, Cycle &c)
         }
         if (many) e->done_cv.notify_all(); else e->done_cv.notify_one();
     }
-    c.streams.clear(); c.is_final.clear(); c.job_packs.clear();
+    c.streams.clear(); c.is_final.clear(); c.job_packs.clear(); c.job_slabs.clear();
     c.njobs = 0; c.bytes = 0; c.busy = false; c.err = cudaSuccess;
 }
 
@@ -1637,6 +1661,8 @@ void disk_feed(dm_engine *e, const std::shared_ptr<Stream> &sp)
     if (!s->disk || s->disk_reads || s->staged.size() + s->jobs_inflight >= 2 || s->suspending || s->lost != DM_OK ||
         s->cuda_failed)
         return;
+    // a ring load also counts the slabs its reader has not finished with: a slow reader slows its own load only
+    if (s->ring && (s->ring->closed || s->ring->held.size() >= s->ring->cap)) return;
     if (s->st != St::Open && s->st != St::Finishing) return;
     uint64_t end = s->staged_to;
     auto it = s->written.upper_bound(s->staged_to);
@@ -1716,6 +1742,7 @@ static void disk_task_read(dm_engine *e, DiskTask &t)
         if (keep) {
             e->st_h2d += t.n;
             s->staged.emplace_back(t.slab, t.n);
+            if (s->ring) s->ring->held.push_back(RingLoad::Held{t.slab, t.off, t.n, false});
             disk_feed(e, t.sp);
         }
         if (keep || s->st == St::Finishing) mark_dirty(e, t.sp, nullptr);
@@ -1736,9 +1763,11 @@ static void disk_task_publish(dm_engine *e, DiskTask &t)
     if (s->check_only) {                        // dm_cache_verify: the verdict is all; the file is the caller's to judge
         if (s->fd >= 0) { close(s->fd); s->fd = -1; }
         s->publishing = false;
+        const bool ring = s->ring && s->st != St::Aborted;
         if (s->st != St::Aborted) s->st = St::Done;
         g.unlock();
         s->cv.notify_all();
+        if (ring) ring_load_settle(e, t.sp);    // (its reader waits for this, not for Done)
         return;
     }
     const bool whole = s->resume_base == 0 ||

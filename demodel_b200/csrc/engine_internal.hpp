@@ -146,6 +146,24 @@ struct Pack {
 
 enum class St { Open, Finishing, Done, Aborted };
 
+// dm_cache_open_verified_ring: a check of a tier file (Stream::check_only, disk-backed) whose read-back slabs also
+// serve its one reader, so the bytes handed out are the bytes the H2D copy took to the kernel and the file is read once.
+// A slab of the load goes back to the ring only when its job has been reaped AND the reader no longer needs it: it read
+// past the slab, its first read started beyond it, or it closed.  Guarded by the stream's mutex.
+struct RingLoad {
+    struct Held { Slab *slab; uint64_t off; uint32_t n; bool reaped; };
+    std::deque<Held> held;        // read back, in file order (staged, hashing, or waiting for the reader)
+    uint32_t cap = 0;             // at most this many slabs out of the ring at once (disk_feed stops issuing reads)
+    uint64_t need = 0;            // the reader needs no byte below this (reads are forward only)
+    uint64_t next = 0;            // the end of the previous read: the next one may not start below it
+    bool started = false;         // the reader's first read has been made (until then nothing is released)
+    bool closed = false;          // dm_cache_close: everything reaped goes back, no further reads are issued
+    bool slot_reserved = true;    // one slot of promote_reserved, until the load ends
+    bool settled = false;         // the verdict has been acted on (drop_corrupt, recency): `status` is final
+    int status = DM_OK;
+    struct stat seen{};           // the file that was read (drop_corrupt)
+};
+
 struct Stream {
     std::mutex mu;
     std::condition_variable cv;
@@ -204,6 +222,7 @@ struct Stream {
     // in a pack as a hash-only member.  It holds no arena extent, and its verdict is all it produces: nothing is
     // published, renamed, truncated or unlinked by the stream (an import publishes its copy itself afterwards).
     bool check_only = false;
+    std::unique_ptr<RingLoad> ring;   // a check that serves a reader (dm_cache_open_verified_ring); set before it is shared
     // A body announced (Content-Length) as at most tiny_max bytes never takes a ring slab: its bytes gather in this
     // private buffer and go straight into a pack when it finishes.  Anything that needs a real slab (more bytes than
     // announced, range parts, zero-copy windows, checkpoints) moves them into one first (take_slab).
@@ -262,6 +281,7 @@ struct Reader {
     std::string disk_meta;        // sidecar text, disk-tier readers (and verified readers until the verdict)
     std::shared_ptr<Stream> follow;   // in-flight body this reader is coalesced onto (until it completes)
     std::shared_ptr<Load> load;       // dm_cache_open_verified of a disk-tier blob: the load `follow` belongs to
+    std::shared_ptr<Stream> ring;     // dm_cache_open_verified_ring of a disk-tier blob: its load (Stream::ring)
     int fd = -1;                  // disk tier; a follower of a disk-backed body: its own descriptor of the body's file
     Digest disk_digest{};         // ... the blob it reads
     bool disk_pin = false;        // ... pinned against disk-tier eviction until dm_cache_close
@@ -382,6 +402,7 @@ struct dm_engine {
     std::mutex slot_mu;              // state / digest slots: a lock of their own, so that opening and closing tiny bodies from
     std::vector<uint32_t> free_slots;                // many threads does not queue on the index lock `mu`
     size_t promote_reserved = 0;     // slots running dm_cache_promote / verify / import calls may take (slot_mu)
+    size_t ring_load_slabs = 0;      // ring slabs the open ring loads may hold (RingLoad::cap each, slot_mu)
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp
     std::unordered_map<Digest, std::weak_ptr<Stream>, DigestHash> inflight;   // open streams by expected digest
@@ -610,6 +631,15 @@ int load_claim(dm_engine *e, const Digest &d, std::shared_ptr<Load> *L);
 int load_begin(dm_engine *e, const std::shared_ptr<Load> &L);
 void load_wake(dm_engine *e);                 // a load's stream completed (complete_stream)
 void load_stop_all(dm_engine *e);             // dm_engine_destroy, while the pump still runs
+
+// Ring loads (dm_cache_open_verified_ring; struct RingLoad).
+// engine_api.cu: start the ring load of a disk-only blob (its check stream finishing, the tier file read in by the disk
+// threads): DM_OK with *sp, *size and *side (the sidecar text), or the open's error with nothing held.
+int ring_load_open(dm_engine *e, const Digest &d, std::shared_ptr<Stream> *sp, uint64_t *size, std::string *side);
+void ring_load_settle(dm_engine *e, const std::shared_ptr<Stream> &sp);   // the verdict is in (disk_task_publish)
+void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp);    // the reader closed: stop, give everything back
+// engine_core.cu, stream mutex held: slabs the reader no longer needs and whose jobs are reaped go back to the ring
+void ring_release(dm_engine *e, const std::shared_ptr<Stream> &sp);
 
 // Disk-tier limit (engine_core.cu).  None takes a stream mutex or may be called with e->mu held.  With no limit set
 // they only count pins; reservations always succeed and nothing is stat'ed, touched or written.

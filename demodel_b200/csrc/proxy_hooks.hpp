@@ -267,13 +267,20 @@ private:
 
 class HitReader {
 public:
-    // verified: Pool.HitVerified (dm_cache_open_verified): a disk-tier blob is served only as the GPU verifies it, and
+    // Verified: Pool.HitVerified (dm_cache_open_verified): a disk-tier blob is served only as the GPU verifies it, and
     // Read returns DM_ECORRUPT / DM_EIO / DM_ECUDA instead of its last byte when it does not hash to its name.
-    HitReader(dm_engine *e, const uint8_t digest[32], bool verified = false) : e_(e)
+    // VerifiedRing: Pool.HitVerifiedRing (dm_cache_open_verified_ring), the same promise without an HBM extent, for
+    // blobs Verified answers with DM_ENOMEM or DM_ESTATE (rc()); its reads go forward only.
+    enum Mode { Plain, Verified, VerifiedRing };
+    HitReader(dm_engine *e, const uint8_t digest[32], Mode mode = Plain) : e_(e)
     {
-        rc_ = verified ? dm_cache_open_verified(e, digest, &id_, &size_) : dm_cache_open(e, digest, &id_, &size_);
+        rc_ = mode == Verified     ? dm_cache_open_verified(e, digest, &id_, &size_)
+              : mode == VerifiedRing ? dm_cache_open_verified_ring(e, digest, &id_, &size_)
+                                     : dm_cache_open(e, digest, &id_, &size_);
         open_ = rc_ == DM_OK;
     }
+    // the bool form is Plain / Verified
+    HitReader(dm_engine *e, const uint8_t digest[32], bool verified) : HitReader(e, digest, verified ? Verified : Plain) {}
     // By request URL: a digest in the URL (OCI) or the alias index (HuggingFace resolve/ URLs).
     HitReader(dm_engine *e, const char *url) : e_(e)
     {
@@ -285,6 +292,7 @@ public:
     uint64_t Release() { open_ = false; return id_; }      // hand the open reader to the caller (C-ABI drivers)
     ~HitReader() { Close(); }
     bool hit() const { return open_; }
+    int rc() const { return rc_; }              // why it is not a hit: DM_ENOENT (a miss) or the open's error
     uint64_t size() const { return size_; }     // Content-Length of the synthesised response
     long Read(void *p, size_t n)
     {

@@ -215,6 +215,23 @@ class Engine:
         check(rc, "dm_cache_open_verified")
         return rid.value, size.value
 
+    def cache_open_verified_ring(self, digest: bytes) -> Optional[tuple[int, int]]:
+        """A verified hit that takes no HBM extent: (reader, size) or None on a miss.
+
+        A blob in HBM opens as with cache_open.  One on the disk tier only is read through pinned ring slabs, hashed on
+        the GPU as dm_cache_verify hashes it, and the reader is served from those slabs: it works for blobs larger than
+        the arena and on engines without an HBM tier.  Reads go forward only (the first may start anywhere; a read
+        below the end of the previous one raises DM_ESTATE), and the read of the last byte (and the EOF read) waits
+        for the verdict.  A mismatch makes that read and every later one raise DM_ECORRUPT (file and sidecar are
+        removed); DM_EIO and DM_ECUDA likewise.  Raises DM_ENOMEM when ring loads hold their share of the ring or no
+        stream slot is to spare, DM_ECORRUPT when the file is not its sidecar's size."""
+        rid, size = C.c_uint64(), C.c_uint64()
+        rc = self._lib.dm_cache_open_verified_ring(self._h, _digest_arg(digest), C.byref(rid), C.byref(size))
+        if rc == DM_ENOENT:
+            return None
+        check(rc, "dm_cache_open_verified_ring")
+        return rid.value, size.value
+
     def cache_follow(self, digest: bytes) -> Optional[tuple[int, int]]:
         """Attach to a body that is still being ingested (request coalescing): (reader, size_hint) or None.
 

@@ -318,15 +318,51 @@ func (p *Pool) Hit(digest *[32]byte) *HitReader {
 // hash to its name.  nil on a miss, and when the blob cannot be loaded
 // (DM_ENOMEM: larger than the arena, no room, no stream slot to spare;
 // DM_ESTATE: a pool without an HBM tier); Hit still serves those, unverified,
-// for a caller that accepts that.
+// for a caller that accepts that, and HitVerifiedRing serves them verified.
 func (p *Pool) HitVerified(digest *[32]byte) *HitReader {
+	r, _ := p.HitVerifiedErr(digest)
+	return r
+}
+
+// HitVerifiedErr is HitVerified that also says why a blob could not be
+// opened: (nil, nil) on a miss, (nil, *Error) otherwise.  An *Error with Code
+// DM_ENOMEM or DM_ESTATE means the blob is cached but cannot be loaded into
+// HBM: serve it with HitVerifiedRing.
+func (p *Pool) HitVerifiedErr(digest *[32]byte) (*HitReader, error) {
 	e := p.engineFor(digest)
 	var id, size C.uint64_t
 	rc := C.dm_cache_open_verified(e, (*C.uint8_t)(unsafe.Pointer(&digest[0])), &id, &size)
-	if rc != C.DM_OK {
-		return nil
+	if rc == C.DM_ENOENT {
+		return nil, nil
 	}
-	return &HitReader{e: e, id: id, Size: int64(size)}
+	if err := check(e, 0, rc); err != nil {
+		return nil, err
+	}
+	return &HitReader{e: e, id: id, Size: int64(size)}, nil
+}
+
+// HitVerifiedRing is a verified hit that takes no HBM extent
+// (dm_cache_open_verified_ring): for blobs larger than the arena, an arena
+// with no room, and pools without an HBM tier.  A blob in HBM opens as with
+// Hit.  One on the disk tier only is read through the engine's pinned ring,
+// hashed on the GPU, and served from the same ring slabs; nothing is placed
+// in HBM, so every such hit hashes the blob again.  Size and the last-byte
+// rule are HitVerified's: the Read that would return the last byte waits for
+// the verdict and returns an *Error (DM_ECORRUPT, DM_EIO, DM_ECUDA) instead
+// on a failure.  Reads go forward only, which io.Copy does.  (nil, nil) on a
+// miss; DM_ENOMEM when ring loads already hold their share of the ring or no
+// stream slot is to spare: retry, or serve with Hit.
+func (p *Pool) HitVerifiedRing(digest *[32]byte) (*HitReader, error) {
+	e := p.engineFor(digest)
+	var id, size C.uint64_t
+	rc := C.dm_cache_open_verified_ring(e, (*C.uint8_t)(unsafe.Pointer(&digest[0])), &id, &size)
+	if rc == C.DM_ENOENT {
+		return nil, nil
+	}
+	if err := check(e, 0, rc); err != nil {
+		return nil, err
+	}
+	return &HitReader{e: e, id: id, Size: int64(size)}, nil
 }
 
 func (r *HitReader) Read(p []byte) (int, error) {

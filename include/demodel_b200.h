@@ -262,6 +262,43 @@ int dm_cache_open(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint
  * Verified serving finishes at one SHA-256 chain's rate per blob (DESIGN.md section 7), where dm_cache_open reads the
  * file at memory speed. */
 int dm_cache_open_verified(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size);
+/* A verified hit that takes no HBM extent: for blobs larger than the arena, an arena with no room, and engines without
+ * an HBM tier (DM_F_NO_HBM_CAS, with or without DM_F_DISK_DIRECT).  Returns at once, without waiting for a load.
+ *   in HBM       exactly dm_cache_open (those bytes were verified when they entered HBM), LRU touch included
+ *   disk only    a ring load starts: the file is read into pinned ring slabs by engine threads, copied from each slab
+ *                to the device and hashed there as a check whose expected digest is the blob's name, as dm_cache_verify
+ *                hashes it, at any size.  The reader copies its bytes straight out of those slabs: the bytes the kernel
+ *                hashes, and the file is read once.  hbm_cas_used, the HBM LRU order and HBM contents do not change.
+ *                *size is the file's size, checked against its sidecar.
+ * Reads of a ring load's reader:
+ *   - forward only.  The first dm_cache_read may start at any offset (a Range: request); after it, each read starts at
+ *     or after the end of the previous one.  A read below that point returns DM_ESTATE (dm_error_detail(reader) says
+ *     why).  The load always hashes from byte 0; slabs below the first read's offset go back as soon as they are hashed.
+ *   - a read blocks until the slab holding `off` has been read back, and returns what is there (possibly less than
+ *     `len`).  NO read returns byte size - 1, nor the EOF at off == size, before the verdict.
+ *   verified     the remaining reads and EOF succeed.  Nothing is published or placed in HBM and the file stays as it
+ *                is; the load counts as a use of the blob for disk-tier recency
+ *   mismatch     that read and every later one return DM_ECORRUPT; file and sidecar are removed if the path still names
+ *                the file that was read, and the digest is a miss
+ *   DM_EIO       the file could not be read or shrank; DM_ECUDA: a copy or launch failed.  The file is left untouched
+ * dm_cache_meta returns the sidecar text read at open; dm_cache_device_extents returns DM_ESTATE (there are no extents).
+ * Each load holds at most 4 ring slabs (two being hashed, two the reader may still need): when the reader falls behind,
+ * its load stops reading the file, and a stalled client slows its own load only, never the pump or other streams.  A
+ * slab goes back to the ring once its job has been reaped and the reader has read past it, started beyond it, or closed.
+ * dm_cache_close before the verdict stops the load: no further reads are issued, its slabs go back as their jobs are
+ * reaped, and its stream slot is released.  Each ring open is a load of its own, not coalesced with other ring opens
+ * or with HBM loads, and dm_cache_follow does not see it: bytes_hashed and h2d_bytes grow by the blob for every ring
+ * open.  The load pins the digest against disk-tier eviction until its verdict and the reader keeps the pin until
+ * dm_cache_close; dm_cache_remove of the digest returns DM_ESTATE while the load runs.
+ * Errors (nothing is opened, the file is left untouched unless DM_ECORRUPT):
+ *   DM_ENOENT    on neither tier
+ *   DM_ECORRUPT  the file is not the size its sidecar states: file and sidecar removed
+ *   DM_EIO       the file could not be opened
+ *   DM_ENOMEM    ring loads already hold their share of the ring (a quarter of its slabs), or no stream slot to spare
+ *                (the budget dm_cache_promote, dm_cache_verify and dm_cache_import share)
+ *   DM_EINVAL    bad arguments
+ * Like dm_cache_open_verified, the last byte arrives at one SHA-256 chain's rate per blob. */
+int dm_cache_open_verified_ring(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size);
 int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t len, size_t *nread);
 /* The blob's sidecar as JSON text: {"digest":"sha256:..","size":N,"encoding":"identity",
  * ..,"headers":{..}}.  *len receives the full length; up to cap-1 bytes + NUL are copied. */
