@@ -137,6 +137,7 @@ SIGNATURES = {
     "dm_cache_list": (C.c_int, [_P, _P, _P, _U64P, C.c_uint32, C.POINTER(C.c_uint32)]),
     "dm_cache_import": (C.c_int, [_P, C.POINTER(C.c_char_p), _P, C.POINTER(C.c_char_p), C.c_uint32, C.c_uint32, _P,
                                   C.POINTER(C.c_int32)]),
+    "dm_cache_export": (C.c_int, [_P, _P, C.POINTER(C.c_char_p), C.c_uint32, C.POINTER(C.c_int32)]),
     "dm_cache_set_disk_limit": (C.c_int, [_P, C.c_uint64]),
     "dm_cache_disk_usage": (C.c_int, [_P, C.POINTER(DmDiskUsage)]),
     "dm_cache_follow": (C.c_int, [_P, _P, _U64P, _U64P]),

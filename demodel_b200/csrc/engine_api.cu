@@ -1271,9 +1271,9 @@ void load_undo(dm_engine *e, Load &L)
 }
 
 // Open the disk copy of `d` for a check: *fd open O_RDONLY, `seen` its fstat, `side` its sidecar text ("" if none).
-// DM_ENOENT without a file (or a cas_dir), DM_EIO when it cannot be opened, DM_ECORRUPT (file and sidecar dropped)
-// when its size is not the one its sidecar states.
-int open_disk_copy(dm_engine *e, const Digest &d, int *fd, struct stat *seen, std::string *side)
+// DM_ENOENT without a file (or a cas_dir), DM_EIO when it cannot be opened, DM_ECORRUPT (file and sidecar dropped
+// unless `keep`) when its size is not the one its sidecar states.
+int open_disk_copy(dm_engine *e, const Digest &d, int *fd, struct stat *seen, std::string *side, bool keep = false)
 {
     *fd = -1;
     if (e->cas_dir.empty()) return DM_ENOENT;
@@ -1291,7 +1291,7 @@ int open_disk_copy(dm_engine *e, const Digest &d, int *fd, struct stat *seen, st
     uint64_t claimed;
     if (!side->empty() && sidecar_size(*side, &claimed) && claimed != (uint64_t)seen->st_size) {
         close(f);
-        drop_corrupt(e, d, *seen);
+        if (!keep) drop_corrupt(e, d, *seen);
         return fail(DM_ECORRUPT, "disk tier file is not the size its sidecar says");
     }
     *fd = f;
@@ -1641,7 +1641,7 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
     return DM_OK;
 }
 
-// ---- checks of files already written (dm_cache_verify, dm_cache_import) -----------------------------------------
+// ---- checks of files already written (dm_cache_verify, dm_cache_import, dm_cache_export) ------------------------
 // A stored file is a disk-backed stream whose every byte is already written.  Each check is an internal stream opened
 // with expect = the digest (when it is known): its fd is the file, [0, size) counts as written, and it is finished at
 // once, so the disk threads read the file back into ring slabs (at most two per check on the hash side) and the pump
@@ -1752,9 +1752,9 @@ int check_verdict(dm_engine *e, Check &c)
     return DM_ECORRUPT;
 }
 
-// What dm_cache_verify and dm_cache_import share: the ring's device mirror (read-backs, and a tiny check that finds
-// no pack, stage slabs there), a slot budget drawn from the reservation dm_cache_promote uses, and kVerifyThreads
-// threads that open checks and collect their verdicts.  The live proxy keeps its ring: at most a quarter of the slabs'
+// What dm_cache_verify, dm_cache_import and dm_cache_export share: the ring's device mirror (read-backs, and a tiny
+// check that finds no pack, stage slabs there), a slot budget drawn from the reservation dm_cache_promote uses, and
+// kVerifyThreads threads that open checks and collect their verdicts.  The live proxy keeps its ring: at most a quarter of the slabs'
 // worth of disk-backed checks are open at once, and each holds at most two slabs.  Ring loads (below) have a quarter of
 // their own, so checks and ring loads together never hold more than half of the ring.
 class CheckRun {
@@ -1999,12 +1999,15 @@ bool on_either_tier(dm_engine *e, const Digest &d)
     return stat(blob_path(e, d.b).c_str(), &st) == 0;
 }
 
-// Copy `src` into a new file `dst`: copy_file_range (a reflink on XFS and btrfs), pread / pwrite where the kernel or
-// the filesystems cannot do that.  Copies up to the end of file as it is now.
-int stage_copy(int src, const std::string &dst)
+// What a failed copy_into says: the source could not be copied, read or written.
+struct StageTexts { const char *copy, *read, *write; };
+constexpr StageTexts kImportTexts = {"could not copy the file into <cas_dir>/incoming", "could not read the file to import",
+                                     "could not write the staged copy under <cas_dir>/incoming"};
+
+// Copy `src` into the new, empty file `out` and close it: copy_file_range (a reflink on XFS and btrfs), pread / pwrite
+// where the kernel or the filesystems cannot do that.  Copies up to the end of file as it is now.
+int copy_into(int src, int out, const StageTexts &t)
 {
-    const int out = open(dst.c_str(), O_CREAT | O_TRUNC | O_WRONLY | O_CLOEXEC, 0644);
-    if (out < 0) return fail(DM_EIO, "could not create the staged copy under <cas_dir>/incoming");
     bool plain = false;
     std::unique_ptr<uint8_t[]> buf;
     constexpr size_t kBuf = 1 << 20;
@@ -2018,7 +2021,7 @@ int stage_copy(int src, const std::string &dst)
             if (r == 0) break;
             if (errno == EINTR) continue;
             if (errno != EXDEV && errno != ENOSYS && errno != EINVAL && errno != EOPNOTSUPP) {
-                rc = fail(DM_EIO, "could not copy the file into <cas_dir>/incoming");
+                rc = fail(DM_EIO, t.copy);
                 break;
             }
             plain = true;
@@ -2026,7 +2029,7 @@ int stage_copy(int src, const std::string &dst)
         }
         const ssize_t r = pread(src, buf.get(), kBuf, off);
         if (r < 0 && errno == EINTR) continue;
-        if (r < 0) { rc = fail(DM_EIO, "could not read the file to import"); break; }
+        if (r < 0) { rc = fail(DM_EIO, t.read); break; }
         if (r == 0) break;
         ssize_t w = 0;
         while (w < r) {
@@ -2035,11 +2038,18 @@ int stage_copy(int src, const std::string &dst)
             if (k <= 0) break;
             w += k;
         }
-        if (w < r) { rc = fail(DM_EIO, "could not write the staged copy under <cas_dir>/incoming"); break; }
+        if (w < r) { rc = fail(DM_EIO, t.write); break; }
         off += r;
     }
-    if (close(out) != 0 && rc == DM_OK) rc = fail(DM_EIO, "could not write the staged copy under <cas_dir>/incoming");
+    if (close(out) != 0 && rc == DM_OK) rc = fail(DM_EIO, t.write);
     return rc;
+}
+
+int stage_copy(int src, const std::string &dst)
+{
+    const int out = open(dst.c_str(), O_CREAT | O_TRUNC | O_WRONLY | O_CLOEXEC, 0644);
+    if (out < 0) return fail(DM_EIO, "could not create the staged copy under <cas_dir>/incoming");
+    return copy_into(src, out, kImportTexts);
 }
 
 // Open the source of `im`, stage it and open the staged file for its check (prepare of CheckRun::run).
@@ -2212,6 +2222,214 @@ static int cache_import_impl(dm_engine *e, const char *const *paths, const uint8
     return DM_OK;
 }
 
+// ---- exporting cached blobs to files (dm_cache_export) ----------------------------------------------------------
+// The other half of an import.  Each blob is copied to a private file next to its destination - out of its HBM extent
+// (held by a reader reference, without touching the LRU order) or, from the disk tier, the way an import stages its
+// source - and that file is checked as an import checks its staged copy, with the digest as the expected value.  Only a
+// file that hashed to its name is renamed over the destination: no byte leaves the cache unless the GPU hashed it.  The
+// cache is only read.  A tier file whose copy fails its check stays where it is: deciding about it is dm_cache_verify's
+// job, and dropping it from here would let a bad destination disk remove good blobs.
+
+namespace {
+
+constexpr StageTexts kExportTexts = {"could not copy the disk tier file to the staged file", "could not read the disk tier file",
+                                     "could not write the staged file next to the destination"};
+constexpr char kExportTag[] = ".dm-export-";
+std::atomic<uint64_t> g_export_id{1};     // per process: engines of one process may export into the same directory
+
+struct Export {
+    const char *dest = nullptr;
+    std::string staged;                   // the private copy, while it exists
+    bool held = false;                    // hold_digest and tier_pin on the digest, from the source copy to the verdict
+};
+
+std::string dir_of(const char *path)      // up to and including the last '/', "" for a name in the working directory
+{
+    const char *slash = strrchr(path, '/');
+    return slash ? std::string(path, (size_t)(slash - path) + 1) : std::string();
+}
+
+// Staged files are .<basename>.dm-export-<pid>-<id>.part in the destination's directory: remove those of processes that
+// are gone (the rule sweep_incoming applies to incoming/), and leave every live process's alone.
+void sweep_export_staging(const std::string &dir)
+{
+    DIR *d = opendir(dir.empty() ? "." : dir.c_str());
+    if (!d) return;
+    while (struct dirent *de = readdir(d)) {
+        const char *name = de->d_name;
+        const size_t n = strlen(name);
+        if (name[0] != '.' || n < 5 || strcmp(name + n - 5, ".part") != 0) continue;
+        const char *tag = nullptr;
+        for (const char *p = strstr(name, kExportTag); p; p = strstr(p + 1, kExportTag)) tag = p;
+        if (!tag) continue;
+        const char *digits = tag + sizeof kExportTag - 1;
+        char *end = nullptr;
+        const long pid = strtol(digits, &end, 10);
+        if (end == digits || *end != '-' || pid <= 0) continue;
+        if (kill((pid_t)pid, 0) == 0 || errno == EPERM) continue;        // alive (EPERM: alive, another user's)
+        unlink((dir + name).c_str());
+    }
+    closedir(d);
+}
+
+void export_release(dm_engine *e, const Check &c, Export &ex)
+{
+    if (!ex.staged.empty()) { unlink(ex.staged.c_str()); ex.staged.clear(); }
+    if (ex.held) { tier_unpin(e, c.d); release_digest(e, c.d); ex.held = false; }
+}
+
+// Copy the blob to its staged file and open that file for its check (prepare of CheckRun::run).  Whatever it leaves
+// held or staged is undone by export_release.
+int export_prepare(dm_engine *e, const CheckRun &run, Check &c, Export &ex, int *fd, std::string *path)
+{
+    struct stat ds;
+    if (stat(ex.dest, &ds) == 0 && S_ISDIR(ds.st_mode)) return fail(DM_EIO, "the destination is a directory");
+    if (const int b = run.blocked()) return b;
+    hold_digest(e, c.d, "a running dm_cache_export");
+    tier_pin(e, c.d);                                    // the tier file is not a disk-tier victim while it is copied
+    ex.held = true;
+    std::shared_ptr<Blob> hbm;
+    std::vector<Extent> ext;
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(c.d);
+        if (it != e->blobs.end() && it->second->in_hbm) {   // verified at ingest; the reference keeps the extent
+            hbm = it->second;
+            hbm->readers++;
+            ext = hbm->extents;
+        }
+    }
+    int src = -1;
+    if (!hbm) {
+        std::string side;
+        const int rc = open_disk_copy(e, c.d, &src, &c.seen, &side, true);
+        if (rc == DM_ECORRUPT)
+            return note_err(e, 0, fail(DM_ECORRUPT, "the disk tier file is not the size its sidecar says: nothing was "
+                                                     "exported, and the file is left to dm_cache_verify"));
+        if (rc != DM_OK) return rc;
+    }
+    mkdirs(ex.dest);
+    ex.staged = dir_of(ex.dest) + "." + (strrchr(ex.dest, '/') ? strrchr(ex.dest, '/') + 1 : ex.dest) + kExportTag +
+                std::to_string((long)getpid()) + "-" + std::to_string(g_export_id.fetch_add(1)) + ".part";
+    int rc = DM_OK;
+    const int out = open(ex.staged.c_str(), O_CREAT | O_EXCL | O_WRONLY | O_CLOEXEC, 0644);
+    if (out < 0) {
+        ex.staged.clear();                               // not ours to unlink
+        rc = fail(DM_EIO, "could not create the staged file next to the destination");
+    }
+    if (hbm) {
+        if (out >= 0) {
+            bool cuda_failed = false;
+            const bool copied = d2h_to_fd(e, ext, hbm->size, out, &cuda_failed);
+            const bool closed = close(out) == 0;
+            if (cuda_failed) rc = fail(DM_ECUDA, "could not copy the blob out of HBM");
+            else if (!copied || !closed) rc = fail(DM_EIO, kExportTexts.write);
+        }
+        std::vector<Extent> gone;
+        { std::lock_guard<std::mutex> g(e->mu); gone = reader_gone(hbm.get()); }
+        if (!gone.empty()) free_extents(e, gone);
+    } else {
+        if (out >= 0) rc = copy_into(src, out, kExportTexts);
+        close(src);
+    }
+    if (rc == DM_OK) {
+        *fd = open(ex.staged.c_str(), O_RDONLY | O_CLOEXEC);
+        if (*fd < 0) rc = fail(DM_EIO, "could not open the staged file");
+        else if (fstat(*fd, &c.seen) != 0) { close(*fd); rc = fail(DM_EIO, "could not stat the staged file"); }
+    }
+    if (rc != DM_OK) return rc;
+    *path = ex.staged;
+    return 1;
+}
+
+// The verdict of an export's check is due: rename the staged file over the destination when it hashed to its name.
+int export_publish(dm_engine *e, Check &c, Export &ex)
+{
+    uint8_t got[32];
+    int matched = 0;
+    const int rc = check_finish(e, c, got, &matched);
+    if (rc != DM_OK) return rc;
+    if (!matched)
+        return note_err(e, 0, fail(DM_ECORRUPT, "the copy of the blob does not hash to its name: nothing was exported, "
+                                                 "and the cache is left as it is (dm_cache_verify decides about the tier file)"));
+    const bool sync = (e->cfg.flags & DM_F_DISK_SYNC) != 0;
+    if (sync) {
+        const int f = open(ex.staged.c_str(), O_RDONLY | O_CLOEXEC);
+        const bool synced = f >= 0 && fsync(f) == 0;
+        if (f >= 0) close(f);
+        if (!synced) return fail(DM_EIO, "could not fsync the staged file");
+    }
+    if (rename(ex.staged.c_str(), ex.dest) != 0) return fail(DM_EIO, "could not rename the staged file over the destination");
+    ex.staged.clear();
+    if (sync) {
+        const std::string dir = dir_of(ex.dest);
+        const int f = open(dir.empty() ? "." : dir.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
+        const bool synced = f >= 0 && fsync(f) == 0;
+        if (f >= 0) close(f);
+        if (!synced) return fail(DM_EIO, "could not fsync the destination's directory");
+    }
+    return DM_OK;
+}
+
+}  // namespace
+
+static int cache_export_impl(dm_engine *e, const uint8_t *digests, const char *const *dest_paths, uint32_t n,
+                             int32_t *status_out)
+{
+    if (!e || (n && (!digests || !dest_paths || !status_out))) return fail(DM_EINVAL, "null argument");
+    std::vector<Check> work;
+    std::vector<Export> exp;
+    std::vector<uint32_t> slot_of(n);
+    {
+        std::unordered_map<std::string, uint32_t> first;       // destination -> its entry: written once, by one digest
+        for (uint32_t i = 0; i < n; ++i) {
+            if (!dest_paths[i]) return fail(DM_EINVAL, "null path");
+            Digest d;
+            memcpy(d.b, digests + 32ull * i, 32);
+            auto ins = first.emplace(dest_paths[i], (uint32_t)work.size());
+            if (ins.second) {
+                work.emplace_back();
+                work.back().d = d;
+                exp.emplace_back();
+                exp.back().dest = dest_paths[i];
+            } else if (!(work[ins.first->second].d == d)) {
+                return fail(DM_EINVAL, "one destination named with two different digests");
+            }
+            slot_of[i] = ins.first->second;
+        }
+    }
+    {
+        std::vector<std::string> dirs;
+        for (const Export &ex : exp) dirs.push_back(dir_of(ex.dest));
+        std::sort(dirs.begin(), dirs.end());
+        dirs.erase(std::unique(dirs.begin(), dirs.end()), dirs.end());
+        for (const std::string &dir : dirs) sweep_export_staging(dir);
+    }
+    // the check of a staged file reads it back through the ring's device mirror on the disk threads, which an engine
+    // without a cas_dir has not started
+    int ring_rc = DM_OK;
+    if (!work.empty() && e->cas_dir.empty()) {
+        ensure_disk_threads(e);
+        ring_rc = ensure_dev_ring(e);
+    }
+    CheckRun run(e, work.size());
+    run.run(work,
+            [&](Check &c, int *fd, std::string *path) -> int {
+                Export &ex = exp[&c - work.data()];
+                const int rc = ring_rc != DM_OK ? ring_rc : export_prepare(e, run, c, ex, fd, path);
+                if (rc != 1) export_release(e, c, ex);
+                return rc;
+            },
+            [&](Check &c, int rc) -> int {
+                Export &ex = exp[&c - work.data()];
+                if (rc == 1) rc = export_publish(e, c, ex);
+                export_release(e, c, ex);
+                return rc;
+            });
+    for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
+    return DM_OK;
+}
+
 // ---- listing the disk tier (dm_cache_list) ----------------------------------------------------------------------
 // Stateless: a page starts strictly after the last digest of the one before, so blobs may come and go between calls.
 // Only the prefix directories from after[0] on are read, one at a time, each sorted on its own.
@@ -2314,6 +2532,10 @@ int dm_cache_import(dm_engine *e, const char *const *paths, const uint8_t *expec
                     uint32_t flags, uint8_t *digests_out, int32_t *status_out)
 {
     return note_err(e, 0, cache_import_impl(e, paths, expect, keys, n, flags, digests_out, status_out));
+}
+int dm_cache_export(dm_engine *e, const uint8_t *digests, const char *const *dest_paths, uint32_t n, int32_t *status_out)
+{
+    return note_err(e, 0, cache_export_impl(e, digests, dest_paths, n, status_out));
 }
 int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, uint64_t *sizes_out, uint32_t cap,
                   uint32_t *n_out)

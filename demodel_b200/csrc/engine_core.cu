@@ -1147,9 +1147,11 @@ void mkdirs(const std::string &path)
 }
 
 // Write the first `size` bytes held in `ext` to `fd` through two pinned buffers: the D2H of piece k+1 runs
-// while piece k is written to the file.  Used by the disk tier (spill) and by dm_stream_suspend.
-bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int fd)
+// while piece k is written to the file.  Used by the disk tier (spill), dm_stream_suspend and dm_cache_export.
+// *cuda_failed (when given): the failure was a copy, not a write.
+bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int fd, bool *cuda_failed)
 {
+    if (cuda_failed) *cuda_failed = false;
     Bounce *bn[2] = {bounce_get(e), bounce_get(e)};
     uint64_t piece_len[2] = {0, 0};
     bool ok = true;
@@ -1162,6 +1164,7 @@ bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int 
             dst += len;
         });
         piece_len[slot] = n;
+        if (err != cudaSuccess && cuda_failed) *cuda_failed = true;
         return err == cudaSuccess;
     };
     uint64_t issued = 0, written = 0;
@@ -1169,7 +1172,11 @@ bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int 
     if (size) { ok = start_piece(0, 0); issued = piece_len[0]; }
     while (ok && written < size) {
         if (issued < size) { ok = start_piece(cur ^ 1, issued); issued += piece_len[cur ^ 1]; }
-        if (cudaStreamSynchronize(bn[cur]->stream) != cudaSuccess) { ok = false; break; }
+        if (cudaStreamSynchronize(bn[cur]->stream) != cudaSuccess) {
+            if (cuda_failed) *cuda_failed = true;
+            ok = false;
+            break;
+        }
         const uint64_t n = piece_len[cur];
         e->st_d2h += n;
         uint64_t w = 0;
@@ -1855,6 +1862,13 @@ void disk_main(dm_engine *e)
         else if (t.kind == DiskTask::Read) disk_task_read(e, t);
         else disk_task_publish(e, t);
     }
+}
+
+void ensure_disk_threads(dm_engine *e)
+{
+    std::lock_guard<std::mutex> g(e->disk_mu);
+    if (!e->disk_threads.empty() || e->disk_stop) return;
+    for (int i = 0; i < kDiskThreads; ++i) e->disk_threads.emplace_back(disk_main, e);
 }
 
 std::shared_ptr<Stream> find_stream(dm_engine *e, uint64_t id)

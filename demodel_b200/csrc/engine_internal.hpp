@@ -2,7 +2,8 @@
 //   engine_core.cu    extents, ring slabs, CAS commit / eviction, the pump (launch decisions), the disk tier
 //   engine_api.cu     C-ABI: engine lifecycle, streams (ingest, ranges, checkpoint / resume, zero-copy windows),
 //                     loads of disk-tier blobs back into HBM (promotion, verified opens), checks of disk-tier files and
-//                     imports of files from outside the cache (internal streams), the listing of the disk tier
+//                     imports of files from outside the cache and exports of cached blobs to files (internal
+//                     streams), the listing of the disk tier
 //   engine_cache.cu   C-ABI: hit serving (readers, followers, verified opens), device-resident ingest, the synthetic
 //                     generator
 // Not installed, not part of the boundary (that is include/demodel_b200.h).
@@ -450,7 +451,7 @@ struct dm_engine {
     std::deque<std::shared_ptr<Blob>> spill_q;
     std::vector<std::thread> spillers;   // kSpillThreads writers of the disk tier
 
-    std::mutex disk_mu;                  // disk threads (any engine with a cas_dir): their queue (taken after a stream mutex, never before)
+    std::mutex disk_mu;                  // disk threads (any engine with a cas_dir, or one that exported): their queue (taken after a stream mutex, never before)
     std::condition_variable disk_cv;
     std::deque<DiskTask> disk_q;
     std::vector<std::weak_ptr<Stream>> disk_starved;   // read-backs that found the ring empty: retried by the disk threads
@@ -593,7 +594,7 @@ Bounce *bounce_get(dm_engine *e);
 Bounce *bounce_try_get(dm_engine *e);     // for long-lived borrowers: leaves a reserve
 void bounce_put(dm_engine *e, Bounce *b);
 void mkdirs(const std::string &path);
-bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int fd);
+bool d2h_to_fd(dm_engine *e, const std::vector<Extent> &ext, uint64_t size, int fd, bool *cuda_failed = nullptr);
 bool spill_one(dm_engine *e, Blob *b);
 void spill_main(dm_engine *e);
 int ensure_dev_ring(dm_engine *e);
@@ -603,6 +604,9 @@ void disk_write(dm_engine *e, const std::shared_ptr<Stream> &sp, Slab *slab, uin
 void disk_feed(dm_engine *e, const std::shared_ptr<Stream> &sp);   // stream mutex held: start the next read-back if one is due
 bool disk_fed(const Stream *s);               // stream mutex held: every byte is written and staged (or never will be)
 void disk_main(dm_engine *e);
+// Engines with a cas_dir start their disk threads at create; one without starts them the first time a check of a file
+// needs them (dm_cache_export).
+void ensure_disk_threads(dm_engine *e);
 std::shared_ptr<Stream> find_stream(dm_engine *e, uint64_t id);
 void drop_stream(dm_engine *e, const std::shared_ptr<Stream> &sp, bool release_slot);
 int ensure_ingest_scratch(dm_engine *e, uint32_t n);

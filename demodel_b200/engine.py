@@ -62,6 +62,7 @@ class Engine:
         check(self._lib.dm_engine_create(C.byref(cfg), C.byref(handle)), "dm_engine_create")
         self._h = handle
         self.device = device
+        self.cas_dir = cas_dir
 
     # -- lifetime ---------------------------------------------------------
     def close(self) -> None:
@@ -349,6 +350,22 @@ class Engine:
                                         c_keys, n, DM_IMP_LINK if link else 0, digs, status), "dm_cache_import")
         raw = bytes(digs)
         return [(status[i], raw[32 * i:32 * i + 32]) for i in range(n)]
+
+    def export(self, digests: Sequence[bytes], paths: Sequence[str]) -> list[int]:
+        """dm_cache_export: write cached blobs to files, each copy hashed on the GPU before it is renamed over
+        paths[i] (missing parent directories are created).  The cache is only read.  One status per entry: DM_OK,
+        DM_ENOENT (on neither tier), DM_ECORRUPT (the copy did not hash to its name; nothing written, the cache left
+        to verify), DM_EIO, DM_ECUDA or DM_ENOMEM.  Raises DM_EINVAL when one path is given two different digests."""
+        digests, paths = list(digests), [os.fsencode(p) for p in paths]
+        if len(digests) != len(paths) or any(len(d) != 32 for d in digests):
+            raise ValueError("one 32-byte digest per path")
+        n = len(paths)
+        c_paths = (C.c_char_p * max(n, 1))(*paths)
+        status = (C.c_int32 * max(n, 1))()
+        blob = b"".join(digests)
+        check(self._lib.dm_cache_export(self._h, C.cast(C.c_char_p(blob), C.c_void_p) if n else None, c_paths, n,
+                                        status), "dm_cache_export")
+        return list(status[:n])
 
     def set_disk_limit(self, limit_bytes: int) -> None:
         """dm_cache_set_disk_limit: keep the disk tier at or under `limit_bytes` (apparent sizes), evicting least

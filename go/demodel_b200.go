@@ -643,6 +643,58 @@ func (p *Pool) Import(files []ImportFile, link bool) ([]int, [][32]byte, error) 
 	return status, digests, first
 }
 
+// ExportFile is one blob for Pool.Export.
+type ExportFile struct {
+	Digest [32]byte // the cached blob
+	Path   string   // the file to write; missing parent directories are created
+}
+
+// Export writes cached blobs to files (dm_cache_export): each blob is copied out of HBM or its disk-tier file into a
+// private file next to Path, hashed on the GPU that owns its digest and renamed over Path only when it hashed to
+// Digest, the engines in parallel.  The cache is only read.  It blocks until every file has a status: 0 (DM_OK) or a
+// negative dm_err - DM_ENOENT (not cached), DM_ECORRUPT (the copy did not hash to its name: nothing written, the tier
+// file is left to Verify), DM_EIO, DM_ECUDA or DM_ENOMEM.  One Path given two different digests is refused before
+// anything is done (DM_EINVAL).
+func (p *Pool) Export(files []ExportFile) ([]int, error) {
+	status := make([]int, len(files))
+	byEngine := make(map[*C.dm_engine][]int)
+	seen := make(map[string][32]byte, len(files))
+	for i := range files {
+		if d, ok := seen[files[i].Path]; ok && d != files[i].Digest {
+			return nil, &Error{Code: int(C.DM_EINVAL), Detail: "one destination named with two different digests: " + files[i].Path}
+		}
+		seen[files[i].Path] = files[i].Digest
+		e := p.engineFor(&files[i].Digest)
+		byEngine[e] = append(byEngine[e], i)
+	}
+	errs := make(chan error, len(byEngine))
+	for e, idx := range byEngine {
+		go func(e *C.dm_engine, idx []int) {
+			paths := make([]*C.char, len(idx)) // C strings: a Go slice of C pointers may be passed to C
+			digests := make([][32]byte, len(idx))
+			for k, i := range idx {
+				paths[k] = C.CString(files[i].Path)
+				digests[k] = files[i].Digest
+			}
+			st := make([]C.int32_t, len(idx))
+			err := check(e, 0, C.dm_cache_export(e, (*C.uint8_t)(unsafe.Pointer(&digests[0][0])),
+				(**C.char)(unsafe.Pointer(&paths[0])), C.uint32_t(len(idx)), &st[0]))
+			for k, i := range idx {
+				status[i] = int(st[k])
+				C.free(unsafe.Pointer(paths[k]))
+			}
+			errs <- err
+		}(e, idx)
+	}
+	var first error
+	for range byEngine {
+		if err := <-errs; err != nil && first == nil {
+			first = err
+		}
+	}
+	return status, first
+}
+
 // List returns up to limit blobs of the disk tier of every engine (dm_cache_list), merged in ascending digest order,
 // strictly after `after` (nil: from the start), with their sizes.  Fewer than limit entries means the listing is
 // complete; the next page starts after the last digest returned.

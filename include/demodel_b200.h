@@ -52,7 +52,8 @@ typedef enum dm_err {
     DM_ERANGE    = -8,   /* offset beyond blob end */
     DM_ECORRUPT  = -9    /* a disk tier copy does not hash to its name (dm_cache_promote, dm_cache_verify,
                           * dm_cache_open_verified and its reads), or a file
-                          * to import does not hash to its expected digest (dm_cache_import) */
+                          * to import does not hash to its expected digest (dm_cache_import), or the copy of a blob
+                          * to export does not (dm_cache_export) */
 } dm_err;
 
 typedef struct dm_engine dm_engine;   /* opaque; owned by caller between create/destroy */
@@ -431,6 +432,39 @@ int dm_cache_list(dm_engine *e, const uint8_t after[32], uint8_t *digests_out, u
  * would refuse, an unknown flag); DM_ESTATE without cas_dir. */
 int dm_cache_import(dm_engine *e, const char *const *paths, const uint8_t *expect, const char *const *keys,
                     uint32_t n, uint32_t flags, uint8_t *digests_out, int32_t *status_out);
+/* Write cached blobs to files the caller names, each checked on the GPU on its way out: the other half of
+ * dm_cache_import (an air-gapped copy, a client's Ollama models directory or HuggingFace hub cache, a second node's
+ * cache, a backup).  Works with or without cas_dir and with DM_F_NO_HBM_CAS.
+ *   digests      n x 32 bytes
+ *   dest_paths   n file names; missing parent directories are created
+ * Entry i is copied from its HBM extent (verified at ingest; a reader reference holds it while it is copied out) or,
+ * when not in HBM, from its disk-tier file (copy_file_range, a reflink on XFS and btrfs; the digest is pinned against
+ * disk-tier eviction meanwhile) into a private file next to the destination, <dir>/.<basename>.dm-export-<pid>-<id>.part,
+ * created with O_EXCL.  That file is hashed on the GPU as dm_cache_import hashes its staged copy, through the ring
+ * (files of at most 64 KiB share pack DMAs and launches), and renamed over dest_paths[i] only when it hashed to
+ * digests[i]: a destination that already exists is replaced atomically (a reader that had it open keeps the old bytes).
+ * On a DM_F_DISK_SYNC engine the file is fsynced before the rename and its directory after it.  On any other outcome
+ * the staged file is unlinked and dest_paths[i] is left as it was.  Blocks until every status is known.  status_out[i]:
+ *   DM_OK        dest_paths[i] holds the blob, and those bytes hashed to digests[i] on the GPU
+ *   DM_ENOENT    on neither tier (a body still being ingested is not cached yet)
+ *   DM_ECORRUPT  the copy did not hash to its name, or the tier file is not its sidecar's size.  Nothing is written at
+ *                dest_paths[i], and the cache is NOT touched: dm_cache_verify decides about the tier file
+ *                (dm_error_detail(e, 0) says so)
+ *   DM_EIO       the source could not be read, or the staged file could not be created, written, synced or renamed
+ *                (a destination that names a directory is one)
+ *   DM_ECUDA     a copy or launch failed
+ *   DM_ENOMEM    no stream slot to spare (the budget dm_cache_promote, dm_cache_verify and dm_cache_import share)
+ * Duplicate (digest, destination) pairs are exported once; each copy gets the status.
+ * The cache is only read: HBM contents, hbm_cas_used, the LRU order, disk-tier recency (the tier file's mtime), the
+ * disk-tier limit's accounting, blobs_committed, blobs_mismatched and bytes_ingested stay as they are.  bytes_hashed
+ * and h2d_bytes grow by the bytes checked, d2h_bytes by the bytes copied out of HBM.
+ * While a call holds a digest (from its source copy until its verdict) dm_cache_remove of it returns DM_ESTATE.
+ * Threads, slot budget and ring share (a quarter of the ring) are dm_cache_verify's, so live streams keep the rest.
+ * Each call first removes, from the directories it writes to, the staged files of processes that are gone.
+ * Returns DM_OK once every status is filled; DM_EINVAL for a null argument or path, or for one destination named with
+ * two different digests (nothing is done then). */
+int dm_cache_export(dm_engine *e, const uint8_t *digests, const char *const *dest_paths, uint32_t n,
+                    int32_t *status_out);
 /* Keep the disk tier under a size limit.  Opt-in: an engine that never sets one touches, scans and reserves nothing.
  * Bytes are apparent sizes (st_size) of the regular files under <cas_dir>/blobs/, incoming/ and partial/
  * (aliases.log is not counted).  A hard-linked import (DM_IMP_LINK) counts at its full size although its inode is
