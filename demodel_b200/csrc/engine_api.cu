@@ -1203,19 +1203,36 @@ static int stream_abort_impl(dm_engine *e, uint64_t id)
 
 namespace {
 
-constexpr int kPromoteThreads = 4;        // loaders: reads of different files overlap
 constexpr int kLoadThreads = 4;           // the engine's loader threads (dm_cache_open_verified)
-// Tiny bodies are flushed this many at a time.  Their hash takes less time than reading the next file, so one by one
-// each would be a launch of its own; together they share a pack DMA and a launch.
-constexpr size_t kPromoteTinyBatch = 256;
 const char *kCorruptText = "the disk tier file does not hash to its digest: file and sidecar removed";
 
-struct Promotion {
-    Digest d;
-    int32_t status = DM_ENOENT;
-    std::shared_ptr<Load> load;           // the load this promotion runs (own), or the running one it waits for
-    bool own = false;
-};
+// The stream slots of the tier calls (dm_cache_promote, verify, import and export, verified opens, ring loads), slot_mu
+// held: take up to `want` of the free slots that no other such call has reserved, at most half of them, so none with
+// one or none left, which stays dm_stream_open's.  Returns how many were taken; slots_release gives them back.
+size_t slots_reserve(dm_engine *e, size_t want)
+{
+    const size_t free = e->free_slots.size();
+    const size_t n = std::min(want, free > e->slots_reserved ? (free - e->slots_reserved) / 2 : 0);
+    e->slots_reserved += n;
+    return n;
+}
+
+void slots_release(dm_engine *e, size_t n)
+{
+    e->slots_reserved -= n;
+}
+
+// pread exactly n bytes at offset 0: false on a read error, or when the file ends first.
+bool pread_full(int fd, uint8_t *buf, uint64_t n)
+{
+    for (uint64_t off = 0; off < n;) {
+        const ssize_t got = pread(fd, buf + off, n - off, (off_t)off);
+        if (got < 0 && errno == EINTR) continue;
+        if (got <= 0) return false;
+        off += (uint64_t)got;
+    }
+    return true;
+}
 
 // The sidecar's top-level "size" (it precedes "headers", so the first match is it).  The number must be followed by
 // ',' or '}': a sidecar read while write_sidecar is still writing it may end in the middle of the number.
@@ -1377,13 +1394,9 @@ int load_fill(dm_engine *e, Load &L, uint8_t *tiny_buf, bool flush_tiny)
     const uint64_t size = L.size;
     const uint64_t id = L.stream;
     int rc = DM_OK;
-    for (uint64_t off = 0; L.tiny && rc == DM_OK && off < size;) {
-        ssize_t got;
-        do got = pread(L.fd, tiny_buf + off, size - off, (off_t)off); while (got < 0 && errno == EINTR);
-        if (got <= 0) { rc = fail(DM_EIO, "could not read the disk tier file"); break; }
-        off += (uint64_t)got;
-        if (off == size) rc = stream_write_impl(e, id, tiny_buf, size);
-    }
+    if (L.tiny && size)
+        rc = pread_full(L.fd, tiny_buf, size) ? stream_write_impl(e, id, tiny_buf, size)
+                                              : fail(DM_EIO, "could not read the disk tier file");
     for (uint64_t off = 0; !L.tiny && rc == DM_OK && off < size;) {
         if (e->load_stop) { rc = fail(DM_ESTATE, "the engine is being destroyed"); break; }
         void *win = nullptr;
@@ -1408,29 +1421,38 @@ int load_fill(dm_engine *e, Load &L, uint8_t *tiny_buf, bool flush_tiny)
     return rc;
 }
 
-// Collect the verdict of a load whose stream is flushed (waits for it): DM_OK with the blob in HBM, DM_ECORRUPT with
-// the file dropped, or the error of a failed copy or launch (the file left untouched).
-int load_verdict(dm_engine *e, Load &L)
+// Collect the digest of a flushed stream that checks a file (waits for it): DM_OK with got[] what the file hashed to,
+// or the error of a failed read, copy or launch (the stream is aborted then).
+int check_finish(dm_engine *e, uint64_t stream, uint8_t got[32], int *matched)
+{
+    const int rc = stream_finish_impl(e, stream, got, matched);
+    if (rc != DM_OK) stream_abort_impl(e, stream);       // (an id finish released just says so)
+    return rc;
+}
+
+// The verdict on the tier file `seen` of `d`, checked by a flushed stream (a load's, or dm_cache_verify's): DM_OK when
+// it hashed to `d` (a load's blob is in HBM then), DM_ECORRUPT with the file dropped, or the error of check_finish with
+// the file left untouched and the entry `load` registered taken back.
+int tier_verdict(dm_engine *e, uint64_t stream, const Digest &d, const struct stat &seen, Load *load = nullptr)
 {
     uint8_t got[32];
     int matched = 0;
-    const int rc = stream_finish_impl(e, L.stream, got, &matched);
+    const int rc = check_finish(e, stream, got, &matched);
     if (rc != DM_OK) {
-        stream_abort_impl(e, L.stream);                  // (an id finish released just says so)
-        load_undo(e, L);
+        if (load) load_undo(e, *load);
         return rc;
     }
     if (matched) return DM_OK;
-    drop_corrupt(e, L.d, L.seen);
+    drop_corrupt(e, d, seen);
     return DM_ECORRUPT;
 }
 
-// The end of a load dm_cache_open_verified began: its slot reservation and disk-tier pin go, a verified blob counts as
+// The end of a load dm_cache_open_verified began: its stream slot and disk-tier pin go, a verified blob counts as
 // used, and the load ends.
 void load_release(dm_engine *e, Load &L, int status)
 {
     const std::string why = status == DM_ECORRUPT ? kCorruptText : g_last_error;
-    if (L.reserved) { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved--; L.reserved = false; }
+    if (L.reserved) { std::lock_guard<std::mutex> g(e->slot_mu); slots_release(e, 1); L.reserved = false; }
     if (status == DM_OK) tier_touch(e, L.d);
     tier_unpin(e, L.d);
     load_end(e, L, status, why.c_str());
@@ -1457,7 +1479,7 @@ void load_main(dm_engine *e)
             for (auto &L : wait) {
                 bool over;
                 { std::lock_guard<std::mutex> gs(L->sp->mu); over = L->sp->st == St::Done || L->sp->st == St::Aborted; }
-                if (over) load_release(e, *L, load_verdict(e, *L));
+                if (over) load_release(e, *L, tier_verdict(e, L->stream, L->d, L->seen, L.get()));
                 else rest.push_back(std::move(L));
             }
             g.lock();
@@ -1476,22 +1498,6 @@ void load_main(dm_engine *e)
             e->load_kick = true;                         // its stream may have completed already
         }
     }
-}
-
-// Claim and start the load of a promotion: DM_OK when the blob is in HBM, 1 when its stream is open and filled (flushed
-// unless tiny), 2 when another load of the digest runs (its verdict is collected at the end of the call), or the
-// promotion's final status.
-int promote_start(dm_engine *e, Promotion &p, uint8_t *tiny_buf, bool may_open)
-{
-    int rc;
-    { std::lock_guard<std::mutex> g(e->mu); rc = load_claim(e, p.d, &p.load); }
-    if (rc != 1) return rc;
-    p.own = true;
-    Load &L = *p.load;
-    rc = load_open(e, L, may_open);
-    if (rc == 1 && (rc = load_fill(e, L, tiny_buf, false)) == DM_OK) return 1;
-    load_end(e, L, rc, g_last_error.c_str());
-    return rc;
 }
 
 }  // namespace
@@ -1514,14 +1520,7 @@ int load_claim(dm_engine *e, const Digest &d, std::shared_ptr<Load> *L)
 
 int load_begin(dm_engine *e, const std::shared_ptr<Load> &L)
 {
-    // one slot of the reservation promotions, checks and imports share: at most half of the free slots nobody has
-    // spoken for, so none with one or none left, which stays dm_stream_open's
-    {
-        std::lock_guard<std::mutex> g(e->slot_mu);
-        const size_t free = e->free_slots.size();
-        L->reserved = free > e->promote_reserved && (free - e->promote_reserved) / 2 >= 1;
-        if (L->reserved) e->promote_reserved++;
-    }
+    { std::lock_guard<std::mutex> g(e->slot_mu); L->reserved = slots_reserve(e, 1) == 1; }
     tier_pin(e, L->d);                                   // not a disk-tier victim until its verdict
     const int rc = load_open(e, *L, L->reserved);
     if (rc != 1) { load_release(e, *L, rc); return rc; }
@@ -1567,72 +1566,139 @@ void load_stop_all(dm_engine *e)
 
 extern "C" {
 
+// ---- batch calls (dm_cache_promote, dm_cache_verify, dm_cache_import, dm_cache_export) ---------------------------
+
+namespace {
+
+constexpr int kBatchThreads = 4;          // threads of a batch call: reads of different files overlap
+// Tiny items are flushed this many at a time.  Their hash takes less time than reading the next file, so one by one
+// each would be a launch of its own; together they share a pack DMA and a launch.
+constexpr size_t kTinyBatch = 256;
+
+// An item of a batch call: a blob to promote or verify, or a file to import or export, and the stream that checks it.
+struct Check {
+    Digest d;                             // the expected digest (when `known`)
+    bool known = true;
+    int32_t status = DM_ENOENT;
+    uint64_t stream = 0;                  // open: the verdict is still to be collected
+    bool tiny = false;                    // in its stream's private buffer until flushed, then in a pack
+    bool disk = false;                    // disk-backed: read back through ring slabs by the disk threads
+    struct stat seen{};                   // the file that was read (st_dev / st_ino), of a check of a file
+};
+
+// One entry per distinct key among the n inputs of a batch call, in order of first appearance: key(i, &k) sets the key
+// of input i or returns the error that fails the call, and add(i) appends the entry of the first input with its key.
+// DM_OK with (*slot_of)[i] the index of input i's entry, or key's error.
+int dedup(uint32_t n, std::vector<uint32_t> *slot_of, const std::function<int(uint32_t, std::string *)> &key,
+          const std::function<void(uint32_t)> &add)
+{
+    std::unordered_map<std::string, uint32_t> first;
+    slot_of->resize(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        std::string k;
+        if (const int rc = key(i, &k)) return rc;
+        auto ins = first.emplace(std::move(k), (uint32_t)first.size());
+        if (ins.second) add(i);
+        (*slot_of)[i] = ins.first->second;
+    }
+    return DM_OK;
+}
+
+// Collects verdicts of a batch thread's open items, oldest first, until it may open one more (`disk`: disk-backed).
+using MakeRoom = std::function<void(bool disk)>;
+
+// The loop of a batch call: up to kBatchThreads threads take the items in turn and open each.  A thread keeps at most
+// budget / threads items open (the call's stream slots), at most disk_share / threads of them disk-backed, flushes tiny
+// ones kTinyBatch at a time and collects verdicts oldest first.
+//   open(c, room, tiny_buf): 1 with c.stream open (c.tiny and c.disk set), or c's final status.  It calls room before
+//     it takes a stream slot.  tiny_buf is tiny_max bytes of the thread's own.
+//   settle(c): c's final status, once c's stream is flushed.
+void run_batch(dm_engine *e, std::vector<Check> &work, size_t budget, size_t disk_share,
+               const std::function<int(Check &, const MakeRoom &, uint8_t *)> &open,
+               const std::function<int(Check &)> &settle)
+{
+    const size_t nthreads = std::min<size_t>({(size_t)kBatchThreads, work.size(), std::max<size_t>(budget, 1), disk_share});
+    const size_t per_thread = std::max<size_t>(1, budget / std::max<size_t>(nthreads, 1));
+    const size_t disk_per_thread = std::max<size_t>(1, disk_share / std::max<size_t>(nthreads, 1));
+    std::atomic<size_t> next{0};
+    auto worker = [&] {
+        cudaSetDevice(e->device);
+        std::vector<uint8_t> tiny_buf(e->tiny_max);
+        std::deque<Check *> opened;                      // verdict not collected yet (oldest first)
+        std::vector<Check *> unflushed;                  // tiny ones among them, flushed together
+        size_t open_disk = 0;
+        // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
+        auto flush = [&] { for (Check *c : unflushed) stream_flush_impl(e, c->stream); unflushed.clear(); };
+        auto collect = [&] {
+            flush();
+            Check *c = opened.front();
+            opened.pop_front();
+            if (c->disk) --open_disk;
+            c->status = settle(*c);
+        };
+        const MakeRoom room = [&](bool disk) {
+            while (!opened.empty() && (opened.size() >= per_thread || (disk && open_disk >= disk_per_thread))) collect();
+        };
+        for (size_t k; (k = next.fetch_add(1)) < work.size();) {
+            Check &c = work[k];
+            const int rc = open(c, room, tiny_buf.data());
+            if (rc != 1) { c.status = rc; continue; }
+            opened.push_back(&c);
+            if (c.tiny) unflushed.push_back(&c);
+            if (c.disk) ++open_disk;
+            if (unflushed.size() >= kTinyBatch) flush();
+        }
+        flush();
+        while (!opened.empty()) collect();
+    };
+    std::vector<std::thread> th;
+    for (size_t t = 1; t < nthreads; ++t) th.emplace_back(worker);
+    if (nthreads) worker();
+    for (auto &t : th) t.join();
+}
+
+}  // namespace
+
 static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, int32_t *status_out)
 {
     if (!e || (n && (!digests || !status_out))) return fail(DM_EINVAL, "null argument");
     if (e->cfg.flags & DM_F_NO_HBM_CAS) return fail(DM_ESTATE, "the engine has no HBM tier (DM_F_NO_HBM_CAS)");
-    std::vector<Promotion> work;
-    std::vector<uint32_t> slot_of(n);
-    {
-        std::unordered_map<Digest, uint32_t, DigestHash> first;
-        for (uint32_t i = 0; i < n; ++i) {
-            Digest d;
-            memcpy(d.b, digests + 32ull * i, 32);
-            auto ins = first.emplace(d, (uint32_t)work.size());
-            if (ins.second) { work.emplace_back(); work.back().d = d; }
-            slot_of[i] = ins.first->second;
-        }
-    }
-    // At most half of the slots that are free and not spoken for by other running calls: 0 with one or none, which
-    // stays dm_stream_open's.
+    std::vector<Check> work;
+    std::vector<uint32_t> slot_of;
+    dedup(n, &slot_of, [&](uint32_t i, std::string *k) { k->assign((const char *)digests + 32ull * i, 32); return DM_OK; },
+          [&](uint32_t i) { work.emplace_back(); memcpy(work.back().d.b, digests + 32ull * i, 32); });
+    std::vector<std::shared_ptr<Load>> loads(work.size());   // the load each promotion runs, or the running one it waits for
     size_t budget;
-    {
-        std::lock_guard<std::mutex> g(e->slot_mu);
-        const size_t free = e->free_slots.size();
-        budget = free > e->promote_reserved ? (free - e->promote_reserved) / 2 : 0;
-        e->promote_reserved += budget;
-    }
-    const size_t nthreads = std::min<size_t>({(size_t)kPromoteThreads, work.size(), std::max<size_t>(budget, 1)});
-    const size_t per_thread = std::max<size_t>(1, budget / std::max<size_t>(nthreads, 1));
-    std::atomic<size_t> next{0};
-    auto loader = [&] {
-        cudaSetDevice(e->device);
-        std::vector<uint8_t> tiny_buf(e->tiny_max);
-        std::deque<Promotion *> open;                    // verdict not collected yet (oldest first)
-        std::vector<Promotion *> unflushed;              // tiny ones among them, flushed together
-        // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
-        auto flush = [&] { for (Promotion *p : unflushed) stream_flush_impl(e, p->load->stream); unflushed.clear(); };
-        auto settle = [&](Promotion &p) {
-            p.status = load_verdict(e, *p.load);
-            load_end(e, *p.load, p.status, p.status == DM_ECORRUPT ? kCorruptText : g_last_error.c_str());
-        };
-        for (size_t k; (k = next.fetch_add(1)) < work.size();) {
-            if (open.size() >= per_thread) {
-                flush();
-                settle(*open.front());
-                open.pop_front();
-            }
-            Promotion &p = work[k];
-            const int rc = promote_start(e, p, tiny_buf.data(), budget > 0);
-            if (rc == 2) continue;                       // another load's: collected below
-            if (rc != 1) { p.status = rc; continue; }
-            open.push_back(&p);
-            if (p.load->tiny) unflushed.push_back(&p);
-            if (unflushed.size() >= kPromoteTinyBatch) flush();
-        }
-        flush();
-        for (Promotion *p : open) settle(*p);
-    };
-    for (Promotion &p : work) hold_digest(e, p.d, "a running dm_cache_promote");
-    for (Promotion &p : work) tier_pin(e, p.d);        // held by this call: not disk-tier victims until it returns
-    std::vector<std::thread> th;
-    for (size_t t = 1; t < nthreads; ++t) th.emplace_back(loader);
-    if (nthreads) loader();
-    for (auto &t : th) t.join();
-    { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved -= budget; }
-    for (Promotion &p : work)                          // a load that was already running reports its own verdict
-        if (p.load && !p.own) p.status = load_wait(*p.load);
-    for (Promotion &p : work) {
+    { std::lock_guard<std::mutex> g(e->slot_mu); budget = slots_reserve(e, SIZE_MAX); }
+    for (Check &p : work) hold_digest(e, p.d, "a running dm_cache_promote");
+    for (Check &p : work) tier_pin(e, p.d);            // held by this call: not disk-tier victims until it returns
+    // A load reads its file into its stream on the calling thread: none is disk-backed, and the ring share is no bound.
+    run_batch(e, work, budget, SIZE_MAX,
+              [&](Check &p, const MakeRoom &room, uint8_t *tiny_buf) -> int {
+                  room(false);
+                  std::shared_ptr<Load> &L = loads[&p - work.data()];
+                  int rc;
+                  { std::lock_guard<std::mutex> g(e->mu); rc = load_claim(e, p.d, &L); }
+                  if (rc != 1) return rc;                // DM_OK: in HBM; 2: another load's, collected below
+                  rc = load_open(e, *L, budget > 0);
+                  if (rc == 1 && (rc = load_fill(e, *L, tiny_buf, false)) == DM_OK) {
+                      p.stream = L->stream;
+                      p.tiny = L->tiny;
+                      return 1;
+                  }
+                  load_end(e, *L, rc, g_last_error.c_str());
+                  return rc;
+              },
+              [&](Check &p) -> int {
+                  Load &L = *loads[&p - work.data()];
+                  const int st = tier_verdict(e, L.stream, L.d, L.seen, &L);
+                  load_end(e, L, st, st == DM_ECORRUPT ? kCorruptText : g_last_error.c_str());
+                  return st;
+              });
+    { std::lock_guard<std::mutex> g(e->slot_mu); slots_release(e, budget); }
+    for (size_t k = 0; k < work.size(); ++k)           // a load that was already running reports its own verdict
+        if (work[k].status == 2) work[k].status = load_wait(*loads[k]);
+    for (Check &p : work) {
         if (p.status == DM_OK) tier_touch(e, p.d);
         tier_unpin(e, p.d);
         release_digest(e, p.d);
@@ -1649,18 +1715,6 @@ static int cache_promote_impl(dm_engine *e, const uint8_t *digests, uint32_t n, 
 // hash-only members, many to a launch.  No check holds an arena extent, and a verdict is all a check produces.
 
 namespace {
-
-constexpr int kVerifyThreads = 4;         // threads that open checks and collect their verdicts
-constexpr size_t kVerifyTinyBatch = 256;  // tiny checks flushed together: they share pack DMAs and launches
-
-struct Check {
-    Digest d;                             // the expected digest (when `known`)
-    bool known = true;
-    int32_t status = DM_ENOENT;
-    uint64_t stream = 0;                  // open: the verdict is still to be collected
-    bool tiny = false;                    // in its stream's private buffer until flushed, then in a pack
-    struct stat seen{};                   // the file that was read (st_dev / st_ino)
-};
 
 bool blob_in_hbm(dm_engine *e, const Digest &d)
 {
@@ -1686,18 +1740,13 @@ int check_open(dm_engine *e, Check &c, int fd, const std::string &path, std::uni
     if (c.tiny) {
         sp->small.reset(new uint8_t[std::max<uint64_t>(size, 1)]);
         sp->small_cap = (uint32_t)size;
-        uint64_t off = 0;
-        while (off < size) {
-            const ssize_t got = pread(fd, sp->small.get() + off, size - off, (off_t)off);
-            if (got < 0 && errno == EINTR) continue;
-            if (got <= 0) break;                         // a read error, or the file shrank since fstat
-            off += (uint64_t)got;
-        }
+        const bool read = pread_full(fd, sp->small.get(), size);    // (false also when the file shrank since fstat)
         close(fd);
-        if (off < size) return fail(DM_EIO, "could not read the disk tier file");
+        if (!read) return fail(DM_EIO, "could not read the disk tier file");
         sp->small_fill = (uint32_t)size;
         sp->received = size;
     } else {
+        c.disk = true;
         sp->disk = true;
         sp->fd = fd;
         sp->path = path;
@@ -1732,42 +1781,26 @@ int check_open(dm_engine *e, Check &c, int fd, const std::string &path, std::uni
     return 1;
 }
 
-// Collect the verdict of an open check: DM_OK with got[] what the file hashed to, or the error of a failed read, copy
-// or launch (the check is aborted then, its file left untouched).
-int check_finish(dm_engine *e, Check &c, uint8_t got[32], int *matched)
+// The ring slabs a batch call's disk-backed checks may hold, and the ones all ring loads together may hold: a quarter
+// of the ring each.
+size_t ring_quarter(dm_engine *e)
 {
-    const int rc = stream_finish_impl(e, c.stream, got, matched);
-    if (rc != DM_OK) stream_abort_impl(e, c.stream);     // (an id finish released just says so)
-    return rc;
-}
-
-int check_verdict(dm_engine *e, Check &c)
-{
-    uint8_t got[32];
-    int matched = 0;
-    const int rc = check_finish(e, c, got, &matched);
-    if (rc != DM_OK) return rc;
-    if (matched) return DM_OK;
-    drop_corrupt(e, c.d, c.seen);
-    return DM_ECORRUPT;
+    return std::max<size_t>(1, e->slab_store.size() / 4);
 }
 
 // What dm_cache_verify, dm_cache_import and dm_cache_export share: the ring's device mirror (read-backs, and a tiny
-// check that finds no pack, stage slabs there), a slot budget drawn from the reservation dm_cache_promote uses, and
-// kVerifyThreads threads that open checks and collect their verdicts.  The live proxy keeps its ring: at most a quarter of the slabs'
-// worth of disk-backed checks are open at once, and each holds at most two slabs.  Ring loads (below) have a quarter of
-// their own, so checks and ring loads together never hold more than half of the ring.
+// check that finds no pack, stage slabs there), the call's stream slots, and run_batch.  The live proxy keeps its ring:
+// at most a quarter of the slabs' worth of disk-backed checks are open at once, and each holds at most two slabs.  Ring
+// loads (below) have a quarter of their own, so checks and ring loads together never hold more than half of the ring.
 class CheckRun {
 public:
     CheckRun(dm_engine *e, size_t n_work) : e_(e)
     {
         ring_ok_ = e->cas_dir.empty() || n_work == 0 || ensure_dev_ring(e) == DM_OK;
         std::lock_guard<std::mutex> g(e->slot_mu);
-        const size_t free = e->free_slots.size();
-        budget_ = free > e->promote_reserved ? (free - e->promote_reserved) / 2 : 0;
-        e->promote_reserved += budget_;
+        budget_ = slots_reserve(e, SIZE_MAX);
     }
-    ~CheckRun() { std::lock_guard<std::mutex> g(e_->slot_mu); e_->promote_reserved -= budget_; }
+    ~CheckRun() { std::lock_guard<std::mutex> g(e_->slot_mu); slots_release(e_, budget_); }
     CheckRun(const CheckRun &) = delete;
     CheckRun &operator=(const CheckRun &) = delete;
 
@@ -1786,48 +1819,18 @@ public:
              const std::function<int(Check &, int)> &settle)
     {
         dm_engine *e = e_;
-        const size_t ring_share = std::max<size_t>(1, e->slab_store.size() / 4);
-        const size_t nthreads = std::min<size_t>({(size_t)kVerifyThreads, work.size(), std::max<size_t>(budget_, 1), ring_share});
-        const size_t per_thread = std::max<size_t>(1, budget_ / std::max<size_t>(nthreads, 1));
-        const size_t disk_per_thread = std::max<size_t>(1, ring_share / std::max<size_t>(nthreads, 1));
-        std::atomic<size_t> next{0};
-        auto checker = [&] {
-            cudaSetDevice(e->device);
-            std::deque<Check *> open;                        // verdict not collected yet (oldest first)
-            std::vector<Check *> unflushed;                  // tiny ones among them, flushed together
-            size_t open_disk = 0;
-            // a flush that fails leaves the stream open: its finish fails the same way and the verdict aborts it
-            auto flush = [&] { for (Check *c : unflushed) stream_flush_impl(e, c->stream); unflushed.clear(); };
-            auto collect = [&] {
-                flush();
-                Check *c = open.front();
-                open.pop_front();
-                if (!c->tiny) --open_disk;
-                c->status = settle(*c, 1);
-            };
-            std::string path;
-            for (size_t k; (k = next.fetch_add(1)) < work.size();) {
-                Check &c = work[k];
-                int fd = -1;
-                const int rc = prepare(c, &fd, &path);
-                if (rc != 1) { c.status = rc; continue; }
-                if (const int b = blocked()) { close(fd); c.status = settle(c, b); continue; }
-                const bool tiny = e->tiny_max && (uint64_t)c.seen.st_size <= e->tiny_max;
-                while (!open.empty() && (open.size() >= per_thread || (!tiny && open_disk >= disk_per_thread))) collect();
-                const int st = check_open(e, c, fd, path);
-                if (st != 1) { c.status = settle(c, st); continue; }
-                open.push_back(&c);
-                if (c.tiny) unflushed.push_back(&c);
-                else ++open_disk;
-                if (unflushed.size() >= kVerifyTinyBatch) flush();
-            }
-            flush();
-            while (!open.empty()) collect();
-        };
-        std::vector<std::thread> th;
-        for (size_t t = 1; t < nthreads; ++t) th.emplace_back(checker);
-        if (nthreads) checker();
-        for (auto &t : th) t.join();
+        run_batch(e, work, budget_, ring_quarter(e),
+                  [&](Check &c, const MakeRoom &room, uint8_t *) -> int {
+                      int fd = -1;
+                      std::string path;
+                      const int rc = prepare(c, &fd, &path);
+                      if (rc != 1) return rc;
+                      if (const int b = blocked()) { close(fd); return settle(c, b); }
+                      room(!(e->tiny_max && (uint64_t)c.seen.st_size <= e->tiny_max));
+                      const int st = check_open(e, c, fd, path);
+                      return st == 1 ? 1 : settle(c, st);
+                  },
+                  [&](Check &c) { return settle(c, 1); });
     }
 
 private:
@@ -1849,17 +1852,9 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
 {
     if (!e || (n && (!digests || !status_out))) return fail(DM_EINVAL, "null argument");
     std::vector<Check> work;
-    std::vector<uint32_t> slot_of(n);
-    {
-        std::unordered_map<Digest, uint32_t, DigestHash> first;
-        for (uint32_t i = 0; i < n; ++i) {
-            Digest d;
-            memcpy(d.b, digests + 32ull * i, 32);
-            auto ins = first.emplace(d, (uint32_t)work.size());
-            if (ins.second) { work.emplace_back(); work.back().d = d; }
-            slot_of[i] = ins.first->second;
-        }
-    }
+    std::vector<uint32_t> slot_of;
+    dedup(n, &slot_of, [&](uint32_t i, std::string *k) { k->assign((const char *)digests + 32ull * i, 32); return DM_OK; },
+          [&](uint32_t i) { work.emplace_back(); memcpy(work.back().d.b, digests + 32ull * i, 32); });
     CheckRun run(e, work.size());
     for (Check &c : work) hold_digest(e, c.d, "a running dm_cache_verify");
     for (Check &c : work) tier_pin(e, c.d);
@@ -1872,7 +1867,7 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
                 *path = blob_path(e, c.d.b);
                 return 1;
             },
-            [&](Check &c, int rc) -> int { return rc == 1 ? check_verdict(e, c) : rc; });
+            [&](Check &c, int rc) -> int { return rc == 1 ? tier_verdict(e, c.stream, c.d, c.seen) : rc; });
     for (Check &c : work) tier_unpin(e, c.d);
     for (Check &c : work) release_digest(e, c.d);
     for (uint32_t i = 0; i < n; ++i) status_out[i] = work[slot_of[i]].status;
@@ -1883,7 +1878,7 @@ static int cache_verify_impl(dm_engine *e, const uint8_t *digests, uint32_t n, i
 // A check of a tier file (above) whose read-back slabs also serve one reader (struct RingLoad).  Each load holds at
 // most kRingLoadSlabs slabs: the two of the hash side (disk_feed) and two that the reader may still be copying from.
 // All ring loads together hold at most a quarter of the ring's slabs (their own quarter: checks have another), and each
-// takes one slot of the reservation dm_cache_promote, dm_cache_verify and dm_cache_import share.
+// takes one stream slot of the tier calls' (slots_reserve).
 
 }  // extern "C"
 
@@ -1893,21 +1888,20 @@ constexpr uint32_t kRingLoadSlabs = 4;
 
 int ring_load_open(dm_engine *e, const Digest &d, std::shared_ptr<Stream> *out, uint64_t *size, std::string *side)
 {
-    const size_t share = std::max<size_t>(1, e->slab_store.size() / 4);
+    const size_t share = ring_quarter(e);
     const uint32_t cap = (uint32_t)std::min<size_t>(kRingLoadSlabs, share);
     {
         std::lock_guard<std::mutex> g(e->slot_mu);
-        const size_t free = e->free_slots.size();
-        if (free <= e->promote_reserved || (free - e->promote_reserved) / 2 < 1)
-            return fail(DM_ENOMEM, "no stream slot to spare for a ring load");
-        if (e->ring_load_slabs + cap > share)
+        if (slots_reserve(e, 1) == 0) return fail(DM_ENOMEM, "no stream slot to spare for a ring load");
+        if (e->ring_load_slabs + cap > share) {
+            slots_release(e, 1);
             return fail(DM_ENOMEM, "the ring slabs ring loads may hold are all taken: retry later, or serve the blob with dm_cache_open");
-        e->promote_reserved++;
+        }
         e->ring_load_slabs += cap;
     }
     auto unreserve = [&] {
         std::lock_guard<std::mutex> g(e->slot_mu);
-        e->promote_reserved--;
+        slots_release(e, 1);
         e->ring_load_slabs -= cap;
     };
     if (const int rc = ensure_dev_ring(e); rc != DM_OK) { unreserve(); return rc; }
@@ -1947,7 +1941,7 @@ void ring_load_settle(dm_engine *e, const std::shared_ptr<Stream> &sp)
         R->status = status;
         R->settled = true;
     }
-    if (unreserve) { std::lock_guard<std::mutex> g(e->slot_mu); e->promote_reserved--; }
+    if (unreserve) { std::lock_guard<std::mutex> g(e->slot_mu); slots_release(e, 1); }
     s->cv.notify_all();
 }
 
@@ -1967,7 +1961,7 @@ void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp)
     // slabs still staged come back from the abort, those being hashed when their jobs are reaped (R->closed)
     if (stop) stream_abort_impl(e, s->id);
     std::lock_guard<std::mutex> g(e->slot_mu);
-    if (unreserve) e->promote_reserved--;
+    if (unreserve) slots_release(e, 1);
     e->ring_load_slabs -= R->cap;
 }
 
@@ -2045,6 +2039,15 @@ int copy_into(int src, int out, const StageTexts &t)
     return rc;
 }
 
+// fsync the file (`dir`: the directory) at `path`: false when it cannot be opened or synced.
+bool fsync_path(const char *path, bool dir = false)
+{
+    const int f = open(path, O_RDONLY | O_CLOEXEC | (dir ? O_DIRECTORY : 0));
+    const bool synced = f >= 0 && fsync(f) == 0;
+    if (f >= 0) close(f);
+    return synced;
+}
+
 int stage_copy(int src, const std::string &dst)
 {
     const int out = open(dst.c_str(), O_CREAT | O_TRUNC | O_WRONLY | O_CLOEXEC, 0644);
@@ -2106,15 +2109,11 @@ int import_prepare(dm_engine *e, const CheckRun &run, uint32_t flags, Check &c, 
 int import_publish(dm_engine *e, Check &c, Import &im)
 {
     int matched = 0;
-    const int rc = check_finish(e, c, im.got, &matched);
+    const int rc = check_finish(e, c.stream, im.got, &matched);
     if (rc != DM_OK) { memset(im.got, 0, 32); return rc; }
     if (!matched) return fail(DM_ECORRUPT, "the file does not hash to the digest it was imported under");
-    if (e->cfg.flags & DM_F_DISK_SYNC) {
-        const int f = open(im.staged.c_str(), O_RDONLY | O_CLOEXEC);
-        const bool synced = f >= 0 && fsync(f) == 0;
-        if (f >= 0) close(f);
-        if (!synced) return fail(DM_EIO, "could not fsync the imported copy");
-    }
+    if ((e->cfg.flags & DM_F_DISK_SYNC) && !fsync_path(im.staged.c_str()))
+        return fail(DM_EIO, "could not fsync the imported copy");
     Digest d;
     memcpy(d.b, im.got, 32);
     const uint64_t size = (uint64_t)c.seen.st_size;
@@ -2182,25 +2181,22 @@ static int cache_import_impl(dm_engine *e, const char *const *paths, const uint8
     static const uint8_t kZero[32] = {0};
     std::vector<Check> work;
     std::vector<Import> imp;
-    std::vector<uint32_t> slot_of(n);
-    {
-        std::unordered_map<std::string, uint32_t> first;       // path and expected digest: a duplicate is imported once
-        for (uint32_t i = 0; i < n; ++i) {
-            const uint8_t *x = expect ? expect + 32ull * i : kZero;
-            std::string key(paths[i]);
-            key.push_back('\0');
-            key.append((const char *)x, 32);
-            auto ins = first.emplace(std::move(key), (uint32_t)work.size());
-            if (ins.second) {
-                work.emplace_back();
-                imp.emplace_back();
-                work.back().known = memcmp(x, kZero, 32) != 0;
-                memcpy(work.back().d.b, x, 32);
-                imp.back().src = paths[i];
-            }
-            slot_of[i] = ins.first->second;
-        }
-    }
+    std::vector<uint32_t> slot_of;
+    auto expected = [&](uint32_t i) { return expect ? expect + 32ull * i : kZero; };
+    dedup(n, &slot_of,
+          [&](uint32_t i, std::string *k) {                    // path and expected digest: a duplicate is imported once
+              *k = paths[i];
+              k->push_back('\0');
+              k->append((const char *)expected(i), 32);
+              return DM_OK;
+          },
+          [&](uint32_t i) {
+              work.emplace_back();
+              imp.emplace_back();
+              work.back().known = memcmp(expected(i), kZero, 32) != 0;
+              memcpy(work.back().d.b, expected(i), 32);
+              imp.back().src = paths[i];
+          });
     CheckRun run(e, work.size());
     run.run(work,
             [&](Check &c, int *fd, std::string *path) -> int {
@@ -2347,27 +2343,18 @@ int export_publish(dm_engine *e, Check &c, Export &ex)
 {
     uint8_t got[32];
     int matched = 0;
-    const int rc = check_finish(e, c, got, &matched);
+    const int rc = check_finish(e, c.stream, got, &matched);
     if (rc != DM_OK) return rc;
     if (!matched)
         return note_err(e, 0, fail(DM_ECORRUPT, "the copy of the blob does not hash to its name: nothing was exported, "
                                                  "and the cache is left as it is (dm_cache_verify decides about the tier file)"));
     const bool sync = (e->cfg.flags & DM_F_DISK_SYNC) != 0;
-    if (sync) {
-        const int f = open(ex.staged.c_str(), O_RDONLY | O_CLOEXEC);
-        const bool synced = f >= 0 && fsync(f) == 0;
-        if (f >= 0) close(f);
-        if (!synced) return fail(DM_EIO, "could not fsync the staged file");
-    }
+    if (sync && !fsync_path(ex.staged.c_str())) return fail(DM_EIO, "could not fsync the staged file");
     if (rename(ex.staged.c_str(), ex.dest) != 0) return fail(DM_EIO, "could not rename the staged file over the destination");
     ex.staged.clear();
-    if (sync) {
-        const std::string dir = dir_of(ex.dest);
-        const int f = open(dir.empty() ? "." : dir.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
-        const bool synced = f >= 0 && fsync(f) == 0;
-        if (f >= 0) close(f);
-        if (!synced) return fail(DM_EIO, "could not fsync the destination's directory");
-    }
+    const std::string dir = dir_of(ex.dest);
+    if (sync && !fsync_path(dir.empty() ? "." : dir.c_str(), true))
+        return fail(DM_EIO, "could not fsync the destination's directory");
     return DM_OK;
 }
 
@@ -2379,25 +2366,25 @@ static int cache_export_impl(dm_engine *e, const uint8_t *digests, const char *c
     if (!e || (n && (!digests || !dest_paths || !status_out))) return fail(DM_EINVAL, "null argument");
     std::vector<Check> work;
     std::vector<Export> exp;
-    std::vector<uint32_t> slot_of(n);
-    {
-        std::unordered_map<std::string, uint32_t> first;       // destination -> its entry: written once, by one digest
-        for (uint32_t i = 0; i < n; ++i) {
+    std::vector<uint32_t> slot_of;
+    std::unordered_map<std::string, const uint8_t *> named;   // destination -> its digest: written once, by one digest
+    const int bad = dedup(
+        n, &slot_of,
+        [&](uint32_t i, std::string *k) -> int {
             if (!dest_paths[i]) return fail(DM_EINVAL, "null path");
-            Digest d;
-            memcpy(d.b, digests + 32ull * i, 32);
-            auto ins = first.emplace(dest_paths[i], (uint32_t)work.size());
-            if (ins.second) {
-                work.emplace_back();
-                work.back().d = d;
-                exp.emplace_back();
-                exp.back().dest = dest_paths[i];
-            } else if (!(work[ins.first->second].d == d)) {
+            const uint8_t *d = digests + 32ull * i;
+            if (memcmp(named.emplace(dest_paths[i], d).first->second, d, 32) != 0)
                 return fail(DM_EINVAL, "one destination named with two different digests");
-            }
-            slot_of[i] = ins.first->second;
-        }
-    }
+            *k = dest_paths[i];
+            return DM_OK;
+        },
+        [&](uint32_t i) {
+            work.emplace_back();
+            memcpy(work.back().d.b, digests + 32ull * i, 32);
+            exp.emplace_back();
+            exp.back().dest = dest_paths[i];
+        });
+    if (bad) return bad;
     {
         std::vector<std::string> dirs;
         for (const Export &ex : exp) dirs.push_back(dir_of(ex.dest));

@@ -159,7 +159,7 @@ struct RingLoad {
     uint64_t next = 0;            // the end of the previous read: the next one may not start below it
     bool started = false;         // the reader's first read has been made (until then nothing is released)
     bool closed = false;          // dm_cache_close: everything reaped goes back, no further reads are issued
-    bool slot_reserved = true;    // one slot of promote_reserved, until the load ends
+    bool slot_reserved = true;    // one of the tier calls' stream slots (slots_reserved), until the load ends
     bool settled = false;         // the verdict has been acted on (drop_corrupt, recency): `status` is final
     int status = DM_OK;
     struct stat seen{};           // the file that was read (drop_corrupt)
@@ -262,7 +262,7 @@ struct Load {
     std::shared_ptr<Blob> mine;           // the disk-only entry this load registered (none if one existed)
     uint64_t stream = 0;
     bool tiny = false;                    // at most tiny_max bytes: read into the stream's private buffer
-    bool reserved = false;                // holds one slot of promote_reserved (a verified open's load)
+    bool reserved = false;                // holds one of the tier calls' stream slots (a verified open's load)
     // published under mu: readers wait here for the stream to open and for the verdict
     std::mutex mu;
     std::condition_variable cv;
@@ -402,7 +402,8 @@ struct dm_engine {
     std::atomic<bool> ring_starved{false};
     std::mutex slot_mu;              // state / digest slots: a lock of their own, so that opening and closing tiny bodies from
     std::vector<uint32_t> free_slots;                // many threads does not queue on the index lock `mu`
-    size_t promote_reserved = 0;     // slots running dm_cache_promote / verify / import calls may take (slot_mu)
+    size_t slots_reserved = 0;       // slots the running tier calls may take: promote, verify, import, export calls,
+                                     // verified opens' loads and ring loads (slots_reserve, slot_mu)
     size_t ring_load_slabs = 0;      // ring slabs the open ring loads may hold (RingLoad::cap each, slot_mu)
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp

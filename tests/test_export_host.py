@@ -76,7 +76,7 @@ for name, fn in sorted(vars(T).items()):
             failed += 1; print("FAIL ", name, kw); traceback.print_exc()
         ran += 1
 print(f"EXPORT MIRROR: {ran} ran, {failed} failed")
-sys.exit(1 if failed or ran < 12 else 0)
+sys.exit(1 if failed or ran < 13 else 0)
 """
 
 

@@ -449,6 +449,26 @@ def test_the_cache_is_unchanged_by_exports(tmp_path):
         _clean(eng)
 
 
+def test_the_last_free_stream_slot_stays_with_dm_stream_open(tmp_path):
+    from demodel_b200 import DM_ENOMEM, DM_OK
+    cas = str(tmp_path / "cas")
+    bodies = [_body(1150, 1000), _body(1151, 2 * SLAB)]
+    out = tmp_path / "out"
+    dests = [str(out / f"f{i}") for i in range(len(bodies))]
+    with _engine(cas, max_streams=3) as eng:
+        digs = _on_disk(eng, tmp_path, bodies)
+        held = [eng.stream_open(None, 0) for _ in range(2)]
+        assert eng.export(digs, dests) == [DM_ENOMEM, DM_ENOMEM]                # one slot free: it is not taken
+        assert not any(os.path.exists(p) for p in dests) and _staged(str(out)) == []
+        last = eng.stream_open(None, 0)
+        for s in held + [last]:
+            eng.stream_abort(s)
+        assert eng.export(digs, dests) == [DM_OK, DM_OK]
+        for d, p in zip(digs, dests):
+            assert _file_hash(p) == d
+        _clean(eng, max_streams=3)
+
+
 def test_stale_staging_files_of_dead_processes_are_swept(tmp_path):
     from demodel_b200 import DM_OK
     cas = str(tmp_path / "cas")
