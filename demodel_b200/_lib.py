@@ -127,6 +127,7 @@ SIGNATURES = {
     "dm_cache_open": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_open_verified": (C.c_int, [_P, _P, _U64P, _U64P]),
     "dm_cache_open_verified_ring": (C.c_int, [_P, _P, _U64P, _U64P]),
+    "dm_cache_open_verified_range": (C.c_int, [_P, _P, C.c_uint64, C.c_uint64, _U64P, _U64P]),
     "dm_cache_read": (C.c_int, [_P, C.c_uint64, C.c_uint64, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "dm_cache_meta": (C.c_int, [_P, C.c_uint64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "dm_cache_close": (C.c_int, [_P, C.c_uint64]),

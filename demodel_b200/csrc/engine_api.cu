@@ -1886,39 +1886,72 @@ namespace dmi {
 
 constexpr uint32_t kRingLoadSlabs = 4;
 
-int ring_load_open(dm_engine *e, const Digest &d, std::shared_ptr<Stream> *out, uint64_t *size, std::string *side)
+static uint32_t ring_load_cap(dm_engine *e)
 {
-    const size_t share = ring_quarter(e);
-    const uint32_t cap = (uint32_t)std::min<size_t>(kRingLoadSlabs, share);
-    {
+    return (uint32_t)std::min<size_t>(kRingLoadSlabs, ring_quarter(e));
+}
+
+int ring_load_reserve(dm_engine *e, size_t n)
+{
+    if (const size_t got = slots_reserve(e, n); got < n) { slots_release(e, got); return 1; }
+    if (e->ring_load_slabs + n * ring_load_cap(e) > ring_quarter(e)) { slots_release(e, n); return 2; }
+    e->ring_load_slabs += n * ring_load_cap(e);
+    return 0;
+}
+
+void ring_load_unreserve(dm_engine *e, size_t n)
+{
+    slots_release(e, n);
+    e->ring_load_slabs -= n * ring_load_cap(e);
+}
+
+int ring_load_open(dm_engine *e, const Digest &d, const std::shared_ptr<RingPart> &part, bool shared, uint64_t off,
+                   uint64_t len, bool reserved, std::shared_ptr<Stream> *out)
+{
+    if (!reserved) {
         std::lock_guard<std::mutex> g(e->slot_mu);
-        if (slots_reserve(e, 1) == 0) return fail(DM_ENOMEM, "no stream slot to spare for a ring load");
-        if (e->ring_load_slabs + cap > share) {
-            slots_release(e, 1);
-            return fail(DM_ENOMEM, "the ring slabs ring loads may hold are all taken: retry later, or serve the blob with dm_cache_open");
-        }
-        e->ring_load_slabs += cap;
+        const int why = ring_load_reserve(e, 1);
+        if (why == 1) return fail(DM_ENOMEM, "no stream slot to spare for a ring load");
+        if (why == 2) return fail(DM_ENOMEM, "the ring slabs ring loads may hold are all taken: retry later, or serve the blob with dm_cache_open");
     }
-    auto unreserve = [&] {
-        std::lock_guard<std::mutex> g(e->slot_mu);
-        slots_release(e, 1);
-        e->ring_load_slabs -= cap;
-    };
+    auto unreserve = [&] { std::lock_guard<std::mutex> g(e->slot_mu); ring_load_unreserve(e, 1); };
     if (const int rc = ensure_dev_ring(e); rc != DM_OK) { unreserve(); return rc; }
-    hold_digest(e, d, "a running ring load (dm_cache_open_verified_ring)");
+    hold_digest(e, d, shared ? "a running shared ring load (dm_cache_open_verified_range)"
+                             : "a running ring load (dm_cache_open_verified_ring)");
     Check c;
     c.d = d;
     int fd = -1;
-    int rc = open_disk_copy(e, d, &fd, &c.seen, side);
+    auto R = std::make_unique<RingLoad>();
+    int rc = open_disk_copy(e, d, &fd, &c.seen, &R->side);
     if (rc == DM_OK) {
-        auto R = std::make_unique<RingLoad>();
-        R->cap = cap;
-        R->seen = c.seen;
-        rc = check_open(e, c, fd, blob_path(e, d.b), std::move(R), out);
+        const uint64_t size = (uint64_t)c.seen.st_size;
+        if (shared && (off > size || len > size - off)) {
+            close(fd);
+            rc = fail(DM_ERANGE, "the range is not within the blob");
+        } else {
+            R->cap = ring_load_cap(e);
+            R->seen = c.seen;
+            R->size = size;
+            R->shared = shared;
+            R->parts.push_back(part);
+            rc = check_open(e, c, fd, blob_path(e, d.b), std::move(R), out);
+        }
     }
     if (rc != 1) { release_digest(e, d); unreserve(); return rc; }
-    *size = (uint64_t)c.seen.st_size;
+    if (shared) {                                               // (unless it has already failed: a tiny file)
+        bool live;
+        { std::lock_guard<std::mutex> g((*out)->mu); live = !(*out)->ring->settled || (*out)->ring->status == DM_OK; }
+        if (live) e->ring_shared.emplace(d, *out);
+    }
     return DM_OK;
+}
+
+// A shared load leaves e->ring_shared (it failed, or its last reader closed)
+static void ring_unlist(dm_engine *e, const std::shared_ptr<Stream> &sp)
+{
+    std::lock_guard<std::mutex> g(e->ring_mu);
+    for (auto [it, end] = e->ring_shared.equal_range(sp->expect); it != end; ++it)
+        if (it->second == sp) { e->ring_shared.erase(it); return; }
 }
 
 void ring_load_settle(dm_engine *e, const std::shared_ptr<Stream> &sp)
@@ -1941,28 +1974,50 @@ void ring_load_settle(dm_engine *e, const std::shared_ptr<Stream> &sp)
         R->status = status;
         R->settled = true;
     }
+    if (R->shared && status != DM_OK) ring_unlist(e, sp);      // (a verified one serves attachments until its last close)
     if (unreserve) { std::lock_guard<std::mutex> g(e->slot_mu); slots_release(e, 1); }
     s->cv.notify_all();
 }
 
-void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp)
+// One reader leaves the load: `part` (attached), or a reader detached from it (nullptr).  The last one stops it.
+static void ring_load_leave(dm_engine *e, const std::shared_ptr<Stream> &sp, const std::shared_ptr<RingPart> &part)
 {
     Stream *s = sp.get();
     RingLoad *R = s->ring.get();
-    bool stop, unreserve;
+    bool last, stop, unreserve = false;
     {
         std::lock_guard<std::mutex> g(s->mu);
-        R->closed = true;
+        if (part) R->parts.erase(std::find(R->parts.begin(), R->parts.end(), part));
+        else R->dependents--;
+        last = R->parts.empty() && R->dependents == 0;
+        R->closed = last;
         ring_release(e, sp);
-        stop = !R->settled && s->st != St::Done && s->st != St::Aborted;
-        unreserve = R->slot_reserved;
-        R->slot_reserved = false;
+        disk_feed(e, sp);                                       // (other readers may be waiting for what it held back)
+        stop = last && !R->settled && s->st != St::Done && s->st != St::Aborted;
+        if (last) { unreserve = R->slot_reserved; R->slot_reserved = false; }
     }
+    if (!last) return;
+    if (R->shared) ring_unlist(e, sp);
     // slabs still staged come back from the abort, those being hashed when their jobs are reaped (R->closed)
     if (stop) stream_abort_impl(e, s->id);
+    s->cv.notify_all();                                         // (readers detached from it may wait for its verdict)
     std::lock_guard<std::mutex> g(e->slot_mu);
     if (unreserve) slots_release(e, 1);
     e->ring_load_slabs -= R->cap;
+}
+
+void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp, const std::shared_ptr<RingPart> &part)
+{
+    bool detached, reservation;
+    {
+        std::lock_guard<std::mutex> g(sp->mu);
+        detached = part->detached;
+        reservation = part->reserved;
+        part->reserved = false;
+    }
+    if (reservation) { std::lock_guard<std::mutex> g(e->slot_mu); ring_load_unreserve(e, 1); }
+    ring_load_leave(e, sp, detached ? nullptr : part);
+    for (const auto &f : part->from) ring_load_leave(e, f, nullptr);
 }
 
 }  // namespace dmi

@@ -146,11 +146,93 @@ static int cache_open_verified_ring_impl(dm_engine *e, const uint8_t digest[32],
     if (!r->blob) {
         if (e->cas_dir.empty()) return DM_ENOENT;
         tier_pin(e, d);                                  // the load's, then the reader's until dm_cache_close
-        const int rc = ring_load_open(e, d, &r->ring, &r->size, &r->disk_meta);
+        auto part = std::make_shared<RingPart>();        // (needs every byte until its first read)
+        const int rc = ring_load_open(e, d, part, false, 0, 0, false, &r->ring);
+        if (rc != DM_OK) { tier_unpin(e, d); return rc; }
+        r->part = part;
+        r->size = r->ring->ring->size;
+        r->disk_meta = r->ring->ring->side;
+        r->disk_digest = d;
+        r->disk_pin = true;
+    }
+    const uint64_t id = e->next_id.fetch_add(1);
+    {
+        std::lock_guard<std::mutex> g(e->reader_mu[id % kStripes]);
+        e->readers[id % kStripes][id] = r;
+    }
+    *reader = id;
+    if (size) *size = r->size;
+    return DM_OK;
+}
+
+// A range open of a disk-only blob: attach to a shared load of `d` that can still serve [off, off + len) (it has not
+// failed and its low-water mark is at most off), or start one.  Every shared load hashes the file from byte 0.  ring_mu is held from
+// the lookup to the start, so concurrent opens of one range never start two loads.
+static int range_attach(dm_engine *e, const Digest &d, Reader *r, uint64_t off, uint64_t len)
+{
+    auto part = std::make_shared<RingPart>();
+    part->started = true;
+    part->need = part->next = off;
+    part->end = len ? off + len : UINT64_MAX;
+    std::lock_guard<std::mutex> g(e->ring_mu);
+    for (auto [it, end] = e->ring_shared.equal_range(d); it != end; ++it) {
+        Stream *s = it->second.get();
+        RingLoad *R = s->ring.get();
+        std::lock_guard<std::mutex> gs(s->mu);
+        if (R->closed || (R->settled ? R->status != DM_OK : s->lost != DM_OK || s->cuda_failed) || R->low > off) continue;
+        if (R->settled) {                               // everything is read: the range must be in the slabs still held
+            uint64_t at = off;
+            const uint64_t stop = std::min<uint64_t>(len ? off + len : R->size, R->size);
+            for (const RingLoad::Held &h : R->held) if (h.off <= at && at < h.off + h.n) at = h.off + h.n;
+            if (at < stop) continue;
+        }
+        if (off > R->size || len > R->size - off) return fail(DM_ERANGE, "the range is not within the blob");
+        R->parts.push_back(part);
+        r->ring = it->second;
+        break;
+    }
+    if (!r->ring) {
+        const int rc = ring_load_open(e, d, part, true, off, len, false, &r->ring);
+        if (rc != DM_OK) return rc;
+    }
+    r->part = part;
+    r->size = r->ring->ring->size;
+    r->disk_meta = r->ring->ring->side;
+    return DM_OK;
+}
+
+// A blob in HBM opens as with dm_cache_open, its reads kept within the range.  One on the disk tier only is served by
+// a shared ring load (range_attach).
+static int cache_open_verified_range_impl(dm_engine *e, const uint8_t digest[32], uint64_t off, uint64_t len,
+                                          uint64_t *reader, uint64_t *size)
+{
+    if (!e || !digest || !reader) return fail(DM_EINVAL, "null argument");
+    Digest d;
+    memcpy(d.b, digest, 32);
+    auto r = std::make_shared<Reader>();
+    r->ranged = true;
+    {
+        std::lock_guard<std::mutex> g(e->mu);
+        auto it = e->blobs.find(d);
+        if (it != e->blobs.end() && it->second->in_hbm) {      // verified when it entered HBM: an ordinary hit
+            const uint64_t n = it->second->size;
+            if (off > n || len > n - off) return fail(DM_ERANGE, "the range is not within the blob");
+            r->blob = it->second;
+            r->blob->readers++;
+            lru_touch(e, r->blob.get());
+            r->size = n;
+        }
+    }
+    if (!r->blob) {
+        if (e->cas_dir.empty()) return DM_ENOENT;
+        tier_pin(e, d);                                  // the reader's, until dm_cache_close
+        const int rc = range_attach(e, d, r.get(), off, len);
         if (rc != DM_OK) { tier_unpin(e, d); return rc; }
         r->disk_digest = d;
         r->disk_pin = true;
     }
+    r->lo = off;
+    r->hi = len ? off + len : r->size;
     const uint64_t id = e->next_id.fetch_add(1);
     {
         std::lock_guard<std::mutex> g(e->reader_mu[id % kStripes]);
@@ -334,52 +416,154 @@ static int follow_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t 
     return DM_OK;
 }
 
-// A read of a ring load's reader (dm_cache_open_verified_ring), forward only.  Waits until the slab holding `off` has been
-// read back, then copies out of it and out of the slabs after it that are already there.  Byte size - 1 and the EOF
-// read wait for the verdict; once it has failed, every read returns its status.
+// How long the slab at a shared load's low-water mark may be held only by readers that are not inside dm_cache_read,
+// while another reader of the load waits for bytes, before those readers are detached (ring_detach; DESIGN.md §4).
+constexpr auto kRangeDetachGrace = std::chrono::milliseconds(500);
+
+// A reader of the shared load `sp` waits for bytes (stream mutex held).  When the slab at the load's low-water mark has
+// been held for kRangeDetachGrace only by readers outside dm_cache_read, and a shared load can be reserved for each of
+// them now, they leave this load (RingPart::detached) and stop holding it back.  Returns when to look again.
+static Clock::time_point ring_detach(dm_engine *e, const std::shared_ptr<Stream> &sp)
+{
+    RingLoad *R = sp->ring.get();
+    const Clock::time_point now = Clock::now();
+    if (R->held.empty() || !R->held.front().reaped) return now + kRangeDetachGrace;
+    const RingLoad::Held &h = R->held.front();
+    Clock::time_point since = h.reaped_at;
+    std::vector<std::shared_ptr<RingPart>> stalled;
+    for (const auto &p : R->parts) {
+        if (!p->needs(h.off, h.n)) continue;
+        if (p->inside) return now + kRangeDetachGrace;
+        stalled.push_back(p);
+        since = std::max(since, p->left);
+    }
+    if (stalled.empty()) return now + kRangeDetachGrace;
+    if (now < since + kRangeDetachGrace) return since + kRangeDetachGrace;
+    {
+        std::lock_guard<std::mutex> g(e->slot_mu);
+        if (ring_load_reserve(e, stalled.size()) != 0) return now + kRangeDetachGrace;   // it keeps pacing this load
+    }
+    for (const auto &p : stalled) {
+        p->detached = p->reserved = true;
+        R->parts.erase(std::find(R->parts.begin(), R->parts.end(), p));
+        R->dependents++;                                    // (it got bytes from this load: see RingPart::from)
+    }
+    ring_release(e, sp);
+    disk_feed(e, sp);
+    return now;
+}
+
+// A reader that was detached (stream mutex of its old load held by g, released here): start the shared load that
+// serves it from now on, with the budget reserved for it when possible.  DM_OK with r->ring / r->part replaced.
+static int ring_rejoin(dm_engine *e, Reader *r, std::unique_lock<std::mutex> &g)
+{
+    RingPart *old = r->part.get();
+    const bool reserved = old->reserved;
+    old->reserved = false;
+    auto part = std::make_shared<RingPart>(*old);
+    part->detached = part->reserved = false;
+    part->from.push_back(r->ring);
+    g.unlock();
+    std::shared_ptr<Stream> sp;
+    int rc;
+    {
+        std::lock_guard<std::mutex> gm(e->ring_mu);
+        rc = ring_load_open(e, r->disk_digest, part, true, part->need, 0, reserved, &sp);
+    }
+    if (rc == DM_ENOENT) return fail(DM_ESTATE, "this reader was detached from a load it held back, and the blob is no longer on the disk tier");
+    if (rc != DM_OK) return rc;
+    old->from.clear();                                      // (the new part holds them now, the old load among them)
+    r->ring = sp;
+    r->part = part;
+    return DM_OK;
+}
+
+// A read of a ring load's reader (dm_cache_open_verified_ring, dm_cache_open_verified_range), forward only.  Waits until
+// the slab holding `off` has been read back, then copies out of it and out of the slabs after it that are already
+// there.  Byte size - 1 and the EOF read wait for the verdict; once it has failed, every read returns its status.
 static int ring_read(dm_engine *e, Reader *r, uint64_t off, void *buf, size_t len, size_t *nread)
 {
     std::lock_guard<std::mutex> gr(r->mu);
-    Stream *s = r->ring.get();
-    RingLoad *R = s->ring.get();
-    if (off > r->size) return fail(DM_ERANGE, "offset beyond blob end");
-    len = (size_t)std::min<uint64_t>(len, r->size - off);
+    if (r->ranged) {
+        if (off < r->lo || off > r->hi) return fail(DM_ERANGE, "this read is outside the range the reader was opened for");
+        len = (size_t)std::min<uint64_t>(len, r->hi - off);
+    } else {
+        if (off > r->size) return fail(DM_ERANGE, "offset beyond blob end");
+        len = (size_t)std::min<uint64_t>(len, r->size - off);
+    }
     const uint64_t gate = r->size ? r->size - 1 : 0;     // bytes from here on wait for the verdict
-    std::unique_lock<std::mutex> g(s->mu);
-    if (R->started && off < R->next)
-        return fail(DM_ESTATE, "a dm_cache_open_verified_ring reader reads forward only: this read starts below the end of the previous one");
-    R->started = true;
-    R->next = off;
-    if (off > R->need) { R->need = off; ring_release(e, r->ring); disk_feed(e, r->ring); }
+    std::unique_lock<std::mutex> g(r->ring->mu);
+    while (r->part->detached) {
+        if (const int rc = ring_rejoin(e, r, g); rc != DM_OK) return rc;
+        g = std::unique_lock<std::mutex>(r->ring->mu);
+    }
+    const std::shared_ptr<Stream> &sp = r->ring;
+    RingLoad *R = sp->ring.get();
+    RingPart *p = r->part.get();
+    // the verdict, once it is in (re-read after the copy below too, which runs unlocked and so may see it arrive): a
+    // failed one is what every later read returns, backward ones included
+    auto failed = [&] {
+        if (p->failed != DM_OK)
+            return fail(p->failed, p->failed == DM_ECORRUPT ? "the disk tier file does not hash to its digest: file and sidecar removed"
+                                                            : "a load this reader was detached from failed");
+        return R->settled && R->status != DM_OK
+                   ? fail(R->status, R->status == DM_ECORRUPT ? "the disk tier file does not hash to its digest: file and sidecar removed"
+                                     : R->status == DM_EIO ? "the disk tier file could not be read" : "a CUDA copy or launch failed while the blob was hashed")
+                   : DM_OK;
+    };
+    if (const int rc = failed(); rc != DM_OK) return rc;
+    if (p->started && off < p->next)
+        return fail(DM_ESTATE, r->ranged ? "a dm_cache_open_verified_range reader reads forward only: this read starts below the end of the previous one"
+                                         : "a dm_cache_open_verified_ring reader reads forward only: this read starts below the end of the previous one");
+    p->started = true;
+    p->next = off;
+    p->inside = true;
+    if (off > p->need) { p->need = off; ring_release(e, sp); disk_feed(e, sp); }
     auto slab_at = [&](uint64_t at) -> const RingLoad::Held * {
         for (const RingLoad::Held &h : R->held) if (at >= h.off && at < h.off + h.n) return &h;
         return nullptr;
     };
-    s->cv.wait(g, [&] { return R->settled || (len == 0 && off < r->size) || (off < gate && slab_at(off)); });
-    if (R->settled && R->status != DM_OK)
-        return fail(R->status, R->status == DM_ECORRUPT ? "the disk tier file does not hash to its digest: file and sidecar removed"
-                             : R->status == DM_EIO ? "the disk tier file could not be read" : "a CUDA copy or launch failed while the blob was hashed");
-    uint8_t *out = static_cast<uint8_t *>(buf);
+    auto ready = [&] { return R->settled || (len == 0 && off < r->size) || (off < gate && slab_at(off)); };
+    if (!R->shared) sp->cv.wait(g, ready);
+    else while (!ready()) sp->cv.wait_until(g, ring_detach(e, sp));    // (the detach timer runs on this waiting thread)
+    int rc = failed();
     size_t done = 0;
-    while (done < len) {
+    uint8_t *out = static_cast<uint8_t *>(buf);
+    while (rc == DM_OK && done < len) {
         const uint64_t at = off + done;
-        const uint64_t limit = R->settled ? r->size : gate;
+        const uint64_t limit = R->settled && R->status == DM_OK ? r->size : gate;   // (a failed verdict keeps the gate)
         const RingLoad::Held *h = at < limit ? slab_at(at) : nullptr;
         if (!h) break;
         const size_t n = (size_t)std::min<uint64_t>(len - done, std::min<uint64_t>(h->off + h->n, limit) - at);
         const uint8_t *src = h->slab->host + (at - h->off);
-        // the slab stays out of the ring while this copy runs: `need` is at most `at`, and only this reader moves it
+        // the slab stays out of the ring while this copy runs: it holds bytes this reader needs (`need` is at most
+        // `at`), only this reader moves its `need`, and a reader inside dm_cache_read is never detached
         g.unlock();
         memcpy(out + done, src, n);
         g.lock();
         done += n;
-        R->next = R->need = off + done;
-        ring_release(e, r->ring);
-        disk_feed(e, r->ring);
+        p->next = p->need = off + done;
+        ring_release(e, sp);
+        disk_feed(e, sp);
     }
-    if (done == 0 && len && R->settled)
-        return fail(DM_ESTATE, "the ring load no longer holds the bytes at this offset");
+    if (rc == DM_OK) rc = failed();                      // a mismatch that arrived during the copy fails this read too
+    if (rc == DM_OK && !p->from.empty() && (off + done > gate || (len == 0 && off == r->size))) {
+        // the last byte or the EOF of a reader that got bytes from loads it was detached from: their verdicts too
+        g.unlock();
+        for (const auto &f : p->from) {
+            std::unique_lock<std::mutex> gf(f->mu);
+            while (!f->ring->settled) f->cv.wait_until(gf, ring_detach(e, f));
+            if ((p->failed = f->ring->status) != DM_OK) break;
+        }
+        g.lock();
+        rc = failed();
+    }
+    if (rc == DM_OK && done == 0 && len && R->settled)
+        rc = fail(DM_ESTATE, "the ring load no longer holds the bytes at this offset");
+    p->inside = false;
+    p->left = Clock::now();
     g.unlock();
+    if (rc != DM_OK) return rc;
     e->st_served += done;
     if (nread) *nread = done;
     return DM_OK;
@@ -416,8 +600,9 @@ static int cache_read_impl(dm_engine *e, uint64_t reader, uint64_t off, void *bu
         int rc = follow_read(e, r.get(), off, buf, len, nread);
         if (rc != 1) return rc;                 // 1: the body completed and was published: fall through to the blob
     }
+    if (r->ranged && (off < r->lo || off > r->hi)) return fail(DM_ERANGE, "this read is outside the range the reader was opened for");
     if (off > r->size) return fail(DM_ERANGE, "offset beyond blob end");
-    len = (size_t)std::min<uint64_t>(len, r->size - off);
+    len = (size_t)std::min<uint64_t>(len, (r->ranged ? r->hi : r->size) - off);
     if (len == 0) return DM_OK;
     uint8_t *out = static_cast<uint8_t *>(buf);
     if (!r->blob) {
@@ -547,7 +732,7 @@ static int cache_close_impl(dm_engine *e, uint64_t reader)
         if (!gone.empty()) free_extents(e, gone);
     }
     if (r->ring) {
-        { std::lock_guard<std::mutex> g(r->mu); ring_load_close(e, r->ring); }
+        { std::lock_guard<std::mutex> g(r->mu); ring_load_close(e, r->ring, r->part); }
         tier_unpin(e, r->disk_digest);
     }
     if (r->fd >= 0) {
@@ -1197,6 +1382,11 @@ int dm_synth_fill_device_many(dm_engine *e, uint64_t seed, uint64_t first_blob, 
 int dm_cache_open(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_impl(e, digest, reader, size)); }
 int dm_cache_open_verified(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_verified_impl(e, digest, reader, size)); }
 int dm_cache_open_verified_ring(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size) { return note_err(e, 0, cache_open_verified_ring_impl(e, digest, reader, size)); }
+int dm_cache_open_verified_range(dm_engine *e, const uint8_t digest[32], uint64_t off, uint64_t len, uint64_t *reader,
+                                 uint64_t *size)
+{
+    return note_err(e, 0, cache_open_verified_range_impl(e, digest, off, len, reader, size));
+}
 int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t len, size_t *nread) { return note_err(e, reader, cache_read_impl(e, reader, off, buf, len, nread)); }
 int dm_cache_meta(dm_engine *e, uint64_t reader, char *buf, size_t cap, size_t *len) { return note_err(e, reader, cache_meta_impl(e, reader, buf, cap, len)); }
 int dm_cache_close(dm_engine *e, uint64_t reader) { return note_err(e, reader, cache_close_impl(e, reader)); }

@@ -720,13 +720,13 @@ void completer_main(dm_engine *e)
 }
 
 // A ring load's slab whose job has been reaped: it no longer comes back by itself (slabs_returning), and goes back to
-// the ring now or once its reader is done with it.  Stream mutex held.
+// the ring now or once its readers are done with it.  Stream mutex held.
 static void ring_reaped(dm_engine *e, const std::shared_ptr<Stream> &sp, Slab *slab)
 {
     e->slabs_returning.fetch_sub(1, std::memory_order_relaxed);
     bool found = false;
     for (RingLoad::Held &h : sp->ring->held)
-        if (h.slab == slab) { h.reaped = found = true; break; }
+        if (h.slab == slab) { h.reaped = found = true; h.reaped_at = Clock::now(); break; }
     if (!found) slab_put(e, slab);              // (not kept: cannot happen, but never lose a slab)
     ring_release(e, sp);
 }
@@ -735,7 +735,11 @@ void ring_release(dm_engine *e, const std::shared_ptr<Stream> &sp)
 {
     RingLoad *R = sp->ring.get();
     for (auto it = R->held.begin(); it != R->held.end();) {
-        if (it->reaped && (R->closed || (R->started && it->off + it->n <= R->need))) {
+        bool needed = false;
+        if (!R->closed)
+            for (const auto &p : R->parts) if (p->needs(it->off, it->n)) { needed = true; break; }
+        if (it->reaped && !needed) {
+            R->low = std::max<uint64_t>(R->low, it->off + it->n);
             slab_put(e, it->slab);
             it = R->held.erase(it);
         } else ++it;

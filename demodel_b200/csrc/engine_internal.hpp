@@ -147,18 +147,48 @@ struct Pack {
 
 enum class St { Open, Finishing, Done, Aborted };
 
-// dm_cache_open_verified_ring: a check of a tier file (Stream::check_only, disk-backed) whose read-back slabs also
-// serve its one reader, so the bytes handed out are the bytes the H2D copy took to the kernel and the file is read once.
-// A slab of the load goes back to the ring only when its job has been reaped AND the reader no longer needs it: it read
-// past the slab, its first read started beyond it, or it closed.  Guarded by the stream's mutex.
-struct RingLoad {
-    struct Held { Slab *slab; uint64_t off; uint32_t n; bool reaped; };
-    std::deque<Held> held;        // read back, in file order (staged, hashing, or waiting for the reader)
-    uint32_t cap = 0;             // at most this many slabs out of the ring at once (disk_feed stops issuing reads)
+using Clock = std::chrono::steady_clock;
+struct Stream;
+
+// One reader attached to a ring load (Reader::part).  Guarded by the mutex of the load's stream.  The reader needs the
+// bytes [need, end) once `started`, and every byte before that.
+struct RingPart {
     uint64_t need = 0;            // the reader needs no byte below this (reads are forward only)
     uint64_t next = 0;            // the end of the previous read: the next one may not start below it
-    bool started = false;         // the reader's first read has been made (until then nothing is released)
-    bool closed = false;          // dm_cache_close: everything reaped goes back, no further reads are issued
+    uint64_t end = UINT64_MAX;    // the end of its range (dm_cache_open_verified_range: off + len)
+    bool started = false;         // the first read has been made, or the range was given at open
+    bool inside = false;          // in dm_cache_read
+    Clock::time_point left = Clock::now();   // when it last left dm_cache_read (or opened)
+    // Taken off a shared load it held back (ring_detach): the load no longer lists it, and its next read starts a
+    // shared load of its own with the budget reserved here (`reserved`, until that load takes it over or the reader closes).
+    bool detached = false, reserved = false;
+    // The loads this reader was detached from (the reader's own, under its mutex).  It got bytes from them, so its last
+    // byte and its EOF wait for their verdicts too, and each keeps running until this reader closes (RingLoad::dependents).
+    std::vector<std::shared_ptr<Stream>> from;
+    int failed = DM_OK;           // ... and one of them failed: every read of the reader returns this (the reader's own)
+    bool needs(uint64_t off, uint64_t n) const { return !started || (off + n > need && off < end); }
+};
+
+// A check of a tier file (Stream::check_only, disk-backed) whose read-back slabs also serve readers, so the bytes
+// handed out are the bytes the H2D copy took to the kernel and the file is read once for all of them.
+//   dm_cache_open_verified_ring: one reader, no other open joins it, and it stops when that reader closes.
+//   dm_cache_open_verified_range: a shared load.  e->ring_shared lists it while it runs; range opens whose range it can
+//   still serve attach to it, and it stops when its last reader closes.
+// A slab of the load goes back to the ring only when its job has been reaped AND no attached reader needs it
+// (RingPart::needs).  Guarded by the stream's mutex.
+struct RingLoad {
+    struct Held { Slab *slab; uint64_t off; uint32_t n; bool reaped; Clock::time_point reaped_at; };
+    std::deque<Held> held;        // read back, in file order (staged, hashing, or waiting for readers)
+    std::vector<std::shared_ptr<RingPart>> parts;   // the attached, open readers
+    uint32_t dependents = 0;      // open readers detached from it (RingPart::from): it stops only when these are gone too
+    uint32_t cap = 0;             // at most this many slabs out of the ring at once (disk_feed stops issuing reads)
+    bool shared = false;          // dm_cache_open_verified_range's
+    // The low-water mark: the end of the last slab given back to the ring (0 before any).  Every byte the load read at
+    // or past it is still held, so a reader whose range starts there or later can attach.
+    uint64_t low = 0;
+    uint64_t size = 0;            // the file's, at open
+    std::string side;             // the sidecar text read at open (dm_cache_meta of every reader)
+    bool closed = false;          // the last reader closed: everything reaped goes back, no further reads are issued
     bool slot_reserved = true;    // one of the tier calls' stream slots (slots_reserved), until the load ends
     bool settled = false;         // the verdict has been acted on (drop_corrupt, recency): `status` is final
     int status = DM_OK;
@@ -282,7 +312,10 @@ struct Reader {
     std::string disk_meta;        // sidecar text, disk-tier readers (and verified readers until the verdict)
     std::shared_ptr<Stream> follow;   // in-flight body this reader is coalesced onto (until it completes)
     std::shared_ptr<Load> load;       // dm_cache_open_verified of a disk-tier blob: the load `follow` belongs to
-    std::shared_ptr<Stream> ring;     // dm_cache_open_verified_ring of a disk-tier blob: its load (Stream::ring)
+    std::shared_ptr<Stream> ring;     // dm_cache_open_verified_ring / _range of a disk-tier blob: its load (Stream::ring)
+    std::shared_ptr<RingPart> part;   // ... and this reader's place in it
+    bool ranged = false;          // dm_cache_open_verified_range: reads stay within [lo, hi)
+    uint64_t lo = 0, hi = 0;
     int fd = -1;                  // disk tier; a follower of a disk-backed body: its own descriptor of the body's file
     Digest disk_digest{};         // ... the blob it reads
     bool disk_pin = false;        // ... pinned against disk-tier eviction until dm_cache_close
@@ -405,6 +438,12 @@ struct dm_engine {
     size_t slots_reserved = 0;       // slots the running tier calls may take: promote, verify, import, export calls,
                                      // verified opens' loads and ring loads (slots_reserve, slot_mu)
     size_t ring_load_slabs = 0;      // ring slabs the open ring loads may hold (RingLoad::cap each, slot_mu)
+    // The running shared ring loads by digest (dm_cache_open_verified_range), more than one per digest after a late
+    // joiner or a detach.  A range open looks up, attaches and starts under ring_mu, so two opens never both start a
+    // load that one could serve.  Lock order: reader.mu → ring_mu → stream.mu; settle and the last close take it
+    // with no stream mutex held.
+    std::mutex ring_mu;
+    std::unordered_multimap<Digest, std::shared_ptr<Stream>, DigestHash> ring_shared;
     std::atomic<uint64_t> next_id{1};
     dm::FlatIndex<Digest, std::shared_ptr<Blob>, DigestHash> blobs;      // guarded by mu; see host_util.hpp
     std::unordered_map<Digest, std::weak_ptr<Stream>, DigestHash> inflight;   // open streams by expected digest
@@ -637,13 +676,21 @@ int load_begin(dm_engine *e, const std::shared_ptr<Load> &L);
 void load_wake(dm_engine *e);                 // a load's stream completed (complete_stream)
 void load_stop_all(dm_engine *e);             // dm_engine_destroy, while the pump still runs
 
-// Ring loads (dm_cache_open_verified_ring; struct RingLoad).
+// Ring loads (dm_cache_open_verified_ring and _range; struct RingLoad).
 // engine_api.cu: start the ring load of a disk-only blob (its check stream finishing, the tier file read in by the disk
-// threads): DM_OK with *sp, *size and *side (the sidecar text), or the open's error with nothing held.
-int ring_load_open(dm_engine *e, const Digest &d, std::shared_ptr<Stream> *sp, uint64_t *size, std::string *side);
+// threads) with `part` as its first reader: DM_OK with *sp (R->size and R->side set), or the open's error with nothing
+// held.  `shared`: a range open's, with ring_mu held; it enters e->ring_shared, and the range [off, off + len) (len 0:
+// to the end) is checked against the file's size (DM_ERANGE).  `reserved`: the slot and ring share were taken by
+// ring_load_reserve (given back here on failure).
+int ring_load_open(dm_engine *e, const Digest &d, const std::shared_ptr<RingPart> &part, bool shared, uint64_t off,
+                   uint64_t len, bool reserved, std::shared_ptr<Stream> *sp);
 void ring_load_settle(dm_engine *e, const std::shared_ptr<Stream> &sp);   // the verdict is in (disk_task_publish)
-void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp);    // the reader closed: stop, give everything back
-// engine_core.cu, stream mutex held: slabs the reader no longer needs and whose jobs are reaped go back to the ring
+// A reader closed: it leaves the load; the last one stops it and gives everything back
+void ring_load_close(dm_engine *e, const std::shared_ptr<Stream> &sp, const std::shared_ptr<RingPart> &part);
+// slot_mu held: the stream slots and ring shares of n new ring loads, all or none: 0, or 1 (no slot) / 2 (no share)
+int ring_load_reserve(dm_engine *e, size_t n);
+void ring_load_unreserve(dm_engine *e, size_t n);                        // slot_mu held
+// engine_core.cu, stream mutex held: slabs no reader needs any more and whose jobs are reaped go back to the ring
 void ring_release(dm_engine *e, const std::shared_ptr<Stream> &sp);
 
 // Disk-tier limit (engine_core.cu).  None takes a stream mutex or may be called with e->mu held.  With no limit set

@@ -271,13 +271,18 @@ public:
     // Read returns DM_ECORRUPT / DM_EIO / DM_ECUDA instead of its last byte when it does not hash to its name.
     // VerifiedRing: Pool.HitVerifiedRing (dm_cache_open_verified_ring), the same promise without an HBM extent, for
     // blobs Verified answers with DM_ENOMEM or DM_ESTATE (rc()); its reads go forward only.
-    enum Mode { Plain, Verified, VerifiedRing };
-    HitReader(dm_engine *e, const uint8_t digest[32], Mode mode = Plain) : e_(e)
+    // VerifiedRange: Pool.HitVerifiedRange (dm_cache_open_verified_range), VerifiedRing's promise for the bytes
+    // [off, off + len) of a Range: request (len 0: to the end), served by a ring load shared with the blob's other range
+    // readers.  Read starts at off and returns 0 at off + len; size() is still the whole blob's (Content-Range).
+    enum Mode { Plain, Verified, VerifiedRing, VerifiedRange };
+    HitReader(dm_engine *e, const uint8_t digest[32], Mode mode = Plain, uint64_t off = 0, uint64_t len = 0) : e_(e)
     {
-        rc_ = mode == Verified     ? dm_cache_open_verified(e, digest, &id_, &size_)
-              : mode == VerifiedRing ? dm_cache_open_verified_ring(e, digest, &id_, &size_)
-                                     : dm_cache_open(e, digest, &id_, &size_);
+        rc_ = mode == Verified       ? dm_cache_open_verified(e, digest, &id_, &size_)
+              : mode == VerifiedRing  ? dm_cache_open_verified_ring(e, digest, &id_, &size_)
+              : mode == VerifiedRange ? dm_cache_open_verified_range(e, digest, off, len, &id_, &size_)
+                                      : dm_cache_open(e, digest, &id_, &size_);
         open_ = rc_ == DM_OK;
+        if (mode == VerifiedRange) off_ = off;
     }
     // the bool form is Plain / Verified
     HitReader(dm_engine *e, const uint8_t digest[32], bool verified) : HitReader(e, digest, verified ? Verified : Plain) {}

@@ -233,6 +233,24 @@ class Engine:
         check(rc, "dm_cache_open_verified_ring")
         return rid.value, size.value
 
+    def cache_open_verified_range(self, digest: bytes, off: int = 0, length: int = 0) -> Optional[tuple[int, int]]:
+        """A verified hit on bytes [off, off + length) of a blob (length 0: to the end): (reader, size) or None on a
+        miss.  `size` is the whole blob's.
+
+        A blob in HBM opens as with cache_open, its reads kept within the range.  One on the disk tier only is served
+        by a shared ring load: the range readers of one blob that a running load can still serve attach to it, so the
+        file is read and hashed once for all of them.  Reads stay within the range (DM_ERANGE otherwise) and go forward
+        only; the read at off + length returns b"", and when that is the blob's end it waits for the verdict, as the
+        read of the last byte does.  A mismatch makes every attached reader's read raise DM_ECORRUPT.  Raises DM_ERANGE
+        when the range is not within the blob, DM_ENOMEM when a new load was needed and none can be reserved."""
+        rid, size = C.c_uint64(), C.c_uint64()
+        rc = self._lib.dm_cache_open_verified_range(self._h, _digest_arg(digest), off, length, C.byref(rid),
+                                                     C.byref(size))
+        if rc == DM_ENOENT:
+            return None
+        check(rc, "dm_cache_open_verified_range")
+        return rid.value, size.value
+
     def cache_follow(self, digest: bytes) -> Optional[tuple[int, int]]:
         """Attach to a body that is still being ingested (request coalescing): (reader, size_hint) or None.
 

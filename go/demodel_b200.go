@@ -365,6 +365,31 @@ func (p *Pool) HitVerifiedRing(digest *[32]byte) (*HitReader, error) {
 	return &HitReader{e: e, id: id, Size: int64(size)}, nil
 }
 
+// HitVerifiedRange is a verified hit on bytes [off, off+length) of a blob
+// (dm_cache_open_verified_range; length 0: to the end), for a `Range:`
+// request.  A blob in HBM opens as with Hit, limited to the range.  A
+// disk-only blob is served from a shared ring load: every range reader of the
+// blob that the load can still serve attaches to it, so N parallel parts of
+// one blob read and hash the file once instead of N times.  Size is the whole
+// blob's size (for Content-Range); Read starts at off and returns io.EOF at
+// off+length, and the Read that would return the blob's last byte waits for
+// the verdict as HitVerifiedRing's does.  (nil, nil) on a miss; DM_ERANGE when
+// the range is not within the blob; DM_ENOMEM only when a new load was needed
+// and ring loads already hold their share of the ring or no stream slot is to
+// spare.
+func (p *Pool) HitVerifiedRange(digest *[32]byte, off, length uint64) (*HitReader, error) {
+	e := p.engineFor(digest)
+	var id, size C.uint64_t
+	rc := C.dm_cache_open_verified_range(e, (*C.uint8_t)(unsafe.Pointer(&digest[0])), C.uint64_t(off), C.uint64_t(length), &id, &size)
+	if rc == C.DM_ENOENT {
+		return nil, nil
+	}
+	if err := check(e, 0, rc); err != nil {
+		return nil, err
+	}
+	return &HitReader{e: e, id: id, Size: int64(size), off: off}, nil
+}
+
 func (r *HitReader) Read(p []byte) (int, error) {
 	if len(p) == 0 {
 		return 0, nil

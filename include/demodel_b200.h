@@ -300,6 +300,47 @@ int dm_cache_open_verified(dm_engine *e, const uint8_t digest[32], uint64_t *rea
  *   DM_EINVAL    bad arguments
  * Like dm_cache_open_verified, the last byte arrives at one SHA-256 chain's rate per blob. */
 int dm_cache_open_verified_ring(dm_engine *e, const uint8_t digest[32], uint64_t *reader, uint64_t *size);
+/* dm_cache_open_verified_range: a verified hit on the byte range [off, off + len) of a blob (len = 0: to the end, as
+ * Range: bytes=off- asks), for the parallel Range: requests in which clients fetch large blobs.  Every reader of a
+ * disk-only blob is served by one SHA-256 check of the tier file shared with every other range reader it can serve,
+ * instead of a ring load of its own.  *size is the whole blob's size.  Errors at open are dm_cache_open_verified_ring's,
+ * plus DM_ERANGE when off > size or off + len > size (nothing is opened).
+ *   in HBM       exactly dm_cache_open (LRU touch included), with reads kept within the range, in any order
+ *   disk only    the reader is served by a shared ring load of the digest: a ring load (as above) whose read-back slabs
+ *                serve every reader attached to it.  The open attaches to a shared load of the digest that has not
+ *                failed and whose low-water mark is at most `off`: the end of the last slab the load gave back to the
+ *                ring (0 before it gave any back), below which it no longer holds what it read (a load whose verdict
+ *                is in only while the slabs it still holds cover the range).  When none can serve it, the open starts
+ *                a new shared load, which hashes the file from byte 0 and which later opens may attach to.
+ * Reads of a range reader:
+ *   - within the range: a read below `off` or past off + len returns DM_ERANGE.  A read at off + len returns 0 bytes:
+ *     the end of the range, and when off + len == size the blob's EOF, which waits for the verdict.
+ *   - of a shared load's reader: forward only, as a ring load's reader's (DM_ESTATE), and blocking until the slab
+ *     holding `off` has been read back.  NO read returns byte size - 1, nor the EOF at off == size, before the verdict.
+ *     Verdicts are a ring load's, for every attached reader at once: on a match the remaining reads succeed and the
+ *     load counts once as a use of the blob; on a mismatch every attached reader gets DM_ECORRUPT on that read and
+ *     every later one, and file and sidecar are removed once; DM_EIO and DM_ECUDA as above.  Every outcome wakes every
+ *     blocked reader.
+ * Pacing: a slab of a shared load goes back to the ring once its job has been reaped and no attached, open reader
+ * still needs it.  A reader needs the slabs that overlap the unread part of its range, [max(off, end of its previous
+ * read), off + len): a reader whose range lies ahead of the load holds nothing and does not slow it.  The load as a
+ * whole holds at most the 4 slabs of a ring load.
+ * Detach: when the slab at a load's low-water mark has been held for a grace time (DESIGN.md §4) only by readers that
+ * are not inside dm_cache_read, while another reader of the load waits for bytes, those stalled readers are detached,
+ * provided a stream slot and ring share can be reserved for each of them at that moment (otherwise they keep pacing the
+ * load).  A detached reader holds nothing of the old load, and its next read is served by a shared load started for it;
+ * its last byte and EOF also wait for the verdict of the load it left, which keeps running until the reader closes.
+ * dm_cache_close of one reader detaches it only; the load stops before its verdict only when its last reader closes.
+ * dm_cache_meta returns the sidecar text read by the open that started the load; dm_cache_device_extents returns
+ * DM_ESTATE.
+ * Budget: each shared load takes one stream slot and a ring load's share of the ring, as a ring load does; a reader
+ * that attaches takes neither, so DM_ENOMEM is returned only when a new load is needed and none can be reserved.
+ * The digest is pinned against disk-tier eviction while a shared load of it runs, and each reader keeps its pin until
+ * dm_cache_close; dm_cache_remove returns DM_ESTATE while a shared load runs.  bytes_hashed and h2d_bytes grow by the
+ * blob once per shared load, bytes_served by what the readers read.  Shared loads and dm_cache_open_verified_ring loads
+ * never attach to each other, and dm_cache_follow sees neither. */
+int dm_cache_open_verified_range(dm_engine *e, const uint8_t digest[32], uint64_t off, uint64_t len,
+                                 uint64_t *reader, uint64_t *size);
 int dm_cache_read(dm_engine *e, uint64_t reader, uint64_t off, void *buf, size_t len, size_t *nread);
 /* The blob's sidecar as JSON text: {"digest":"sha256:..","size":N,"encoding":"identity",
  * ..,"headers":{..}}.  *len receives the full length; up to cap-1 bytes + NUL are copied. */
